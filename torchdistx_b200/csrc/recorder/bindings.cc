@@ -41,11 +41,16 @@ void py_leave_fake_mode() {
     torch::utils::set_requires_device_init(at::kCUDA, true);
 }
 
+tdx::RngStream rng_stream(const std::string& rng) {
+  if (rng == "aten") return tdx::RngStream::Aten;
+  if (rng != "fused") throw py::value_error("rng must be \"fused\" or \"aten\", got \"" + rng + "\"");
+  return tdx::RngStream::Fused;
+}
+
 tdx::MaterializeOptions make_options(const py::object& device, const py::object& shard, bool fused,
                                      const std::string& rng = "fused") {
   tdx::MaterializeOptions o;
-  if (rng == "aten") o.rng = tdx::RngStream::Aten;
-  else if (rng != "fused") throw py::value_error("rng must be \"fused\" or \"aten\", got \"" + rng + "\"");
+  o.rng = rng_stream(rng);
   if (!device.is_none()) o.device = py::cast<c10::Device>(device);
   if (!shard.is_none()) {
     auto t = py::cast<std::pair<int64_t, int64_t>>(shard);
@@ -418,8 +423,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("materialize_flat_shard", &py_materialize_flat_shard, py::arg("tensors"), py::arg("rank"), py::arg("world"),
         py::arg("align_numel") = 0, py::arg("device") = py::none(), py::arg("out") = py::none(),
         py::arg("rng") = "fused");
-  m.def("plan_info", [](const at::Tensor& t) {
-    const tdx::PlanInfo i = tdx::plan_info(t);
+  m.def("plan_info", [](const at::Tensor& t, const std::string& rng) {
+    const tdx::PlanInfo i = tdx::plan_info(t, rng_stream(rng));
     py::dict d;
     d["deferred"] = i.deferred;
     d["fusible"] = i.fusible;
@@ -467,11 +472,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       sd["band_hi"] = g.band_hi;
       sd["band_in"] = g.band_in;
       sd["band_out"] = g.band_out;
+      if (rng == "aten") sd["aten_wide"] = g.aten_wide;
       segs.append(sd);
     }
     d["segments"] = segs;
+    if (rng == "aten") d["aten_refusal"] = i.aten_refusal;
     return d;
-  });
+  }, py::arg("tensor"), py::arg("rng") = "fused");
   m.def("_drain", [] {
     py::gil_scoped_release nogil;  // the helper may need the GIL to let go of Python objects
     tdx::drain_background();

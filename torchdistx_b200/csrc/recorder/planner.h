@@ -222,6 +222,9 @@ struct PlanSegment {
   // band_in when band_lo <= c - r <= band_hi and band_out otherwise (little-endian element bits)
   int64_t band_rows = 0, band_cols = 0, band_lo = 0, band_hi = 0;
   uint64_t band_in = 0, band_out = 0;
+  // RngStream::Aten, a drawn segment: the draw ran on fp32 and is rounded at the store
+  // (TDX_ALGO_ATEN_WIDE), whether or not anything can observe the fp32 tensor -- unlike `wide`
+  bool aten_wide = false;
 };
 
 struct PlanInfo {
@@ -249,8 +252,12 @@ struct PlanInfo {
   // the tensor as a list of disjoint segments (one for a tensor initialised as a whole; three for
   // `w.normal_(); w[padding_idx].zero_()`); the scalar fields above describe the largest one
   std::vector<PlanSegment> segments;
+  // RngStream::Aten: why ATen's stream cannot take the storage's random program ("": it can; then
+  // `fusible` is the default stream's verdict, else false).  Computed without a device: the grid
+  // stride a draw takes depends on the device that materialises it.
+  std::string aten_refusal;
 };
-PlanInfo plan_info(const at::Tensor& fake);
+PlanInfo plan_info(const at::Tensor& fake, RngStream rng = RngStream::Fused);
 // Every recorded op touching the tensor's storage, in order (debug aid for unfusable programs).
 std::vector<std::string> storage_history(const at::Tensor& fake);
 

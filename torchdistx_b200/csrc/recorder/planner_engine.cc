@@ -430,32 +430,12 @@ at::Tensor alias_of(const at::Tensor& base, const ValueInfo& v, bool first) {
 }
 
 // Under RngStream::Aten a storage takes the kernels only if ATen launches every draw on it, live or
-// dead, as one 32-bit, trivially 1-D iterator (a contiguous tensor, N < 2^31, 1 + (N - 1) * itemsize <
-// 2^31: TensorIteratorBase::can_use_32bit_indexing), and if every epilogue step of a drawn segment is
-// one the kernels compute bit for bit as ATen's CUDA op does.  Everything else is replayed through ATen.
-bool aten_exact_step(uint32_t op) {
-  switch (op & 0xffu) {
-    case TDX_EPI_MUL: case TDX_EPI_ADD: case TDX_EPI_ERFINV: case TDX_EPI_CLAMP: case TDX_EPI_EXP:
-    case TDX_EPI_LOG: case TDX_EPI_EXPM1: case TDX_EPI_INV_SOFTPLUS: case TDX_EPI_MULADD:
-      return true;
-    default:
-      return false;
-  }
-}
+// dead, as one 32-bit, trivially 1-D iterator, and if every epilogue step of a drawn segment is one
+// the kernels compute bit for bit as ATen's CUDA op does (planner_eval.cc aten_draw_refusal,
+// aten_exact_step; plan_info(rng="aten") reports the same verdict).  Everything else is replayed
+// through ATen.
 bool aten_fusible(const Tape& tape, const StorageTemplate& t) {
-  constexpr int64_t kMax32 = (int64_t{1} << 31) - 1;
-  for (const RngPass& r : t.st.rng_chain) {
-    const TapeOp& op = tape.ops[r.op];
-    if (op.outputs.empty() || op.outputs[0] == kNoValue) return false;
-    const ValueInfo& v = tape.values[op.outputs[0]];
-    const int64_t isz = static_cast<int64_t>(c10::elementSize(v.dtype));
-    if (v.numel != r.numel || v.numel > kMax32 || (v.numel > 0 && (v.numel - 1) > (kMax32 - 1) / isz)) return false;
-    int64_t expect = 1;
-    for (size_t k = v.sizes.size(); k-- > 0;) {
-      if (v.sizes[k] != 1 && v.strides[k] != expect) return false;
-      expect *= v.sizes[k];
-    }
-  }
+  if (!aten_draw_refusal(tape, t.st.rng_chain).empty()) return false;
   for (const FastSeg& sg : t.segs) {
     if (sg.rng_slot == kNoValue) continue;
     for (int i = 0; i < sg.proto.n_epi; ++i)

@@ -1281,6 +1281,39 @@ bool wide_observable(const Tape& tape, const Sym& sy) {
   return false;
 }
 
+// ATen launches a draw as one trivially 1-D iterator with 32-bit indexing when it runs on a contiguous
+// tensor with N < 2^31 and 1 + (N - 1) * itemsize < 2^31 (TensorIteratorBase::can_use_32bit_indexing).
+std::string aten_draw_refusal(const Tape& tape, const RngChain& chain) {
+  constexpr int64_t kMax32 = (int64_t{1} << 31) - 1;
+  for (const RngPass& r : chain) {
+    const TapeOp& op = tape.ops[r.op];
+    const std::string name = op.name();
+    if (op.outputs.empty() || op.outputs[0] == kNoValue) return name + " has no recorded result";
+    const ValueInfo& v = tape.values[op.outputs[0]];
+    const int64_t isz = static_cast<int64_t>(c10::elementSize(v.dtype));
+    if (v.numel != r.numel) return name + " drew on a tensor of another size";
+    if (v.numel > kMax32 || (v.numel > 0 && (v.numel - 1) > (kMax32 - 1) / isz))
+      return name + " of " + std::to_string(v.numel) + " " + c10::toString(v.dtype) +
+             " elements needs 64-bit indexing";
+    int64_t expect = 1;
+    for (size_t k = v.sizes.size(); k-- > 0;) {
+      if (v.sizes[k] != 1 && v.strides[k] != expect) return name + " drew through a non-contiguous view";
+      expect *= v.sizes[k];
+    }
+  }
+  return "";
+}
+
+bool aten_exact_step(uint32_t op) {
+  switch (op & 0xffu) {
+    case TDX_EPI_MUL: case TDX_EPI_ADD: case TDX_EPI_ERFINV: case TDX_EPI_CLAMP: case TDX_EPI_EXP:
+    case TDX_EPI_LOG: case TDX_EPI_EXPM1: case TDX_EPI_INV_SOFTPLUS: case TDX_EPI_MULADD:
+      return true;
+    default:
+      return false;
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
 // lowering: a State as descriptors
 // ---------------------------------------------------------------------------------------------
@@ -1420,7 +1453,7 @@ bool build_fast(const StorageInfo& si, StorageTemplate& t, bool may_sync) {
   return true;
 }
 
-PlanInfo plan_info(const at::Tensor& fake) {
+PlanInfo plan_info(const at::Tensor& fake, RngStream rng) {
   PlanInfo info;
   if (!can_materialize(fake)) {
     info.source = "real";
@@ -1504,6 +1537,7 @@ PlanInfo plan_info(const at::Tensor& fake) {
     ps.p0 = g.st.p0;
     ps.p1 = g.st.p1;
     ps.wide = wide_observable(tape, g.st);
+    ps.aten_wide = rng == RngStream::Aten && g.st.rng() && g.st.wide;
     ps.src_noround = g.st.src_noround;
     if (g.st.src == Sym::Gather) {
       ps.gather_period = g.st.period;
@@ -1538,6 +1572,22 @@ PlanInfo plan_info(const at::Tensor& fake) {
       if (&g == main) info.const_bytes = ps.const_bytes;
     }
     info.segments.push_back(std::move(ps));
+  }
+  if (rng == RngStream::Aten) {  // (the engine's aten_fusible, on the same chain and epilogues)
+    static const char* steps[] = {"?", "mul", "add", "erfinv", "clamp", "pow", "reciprocal", "exp", "log", "expm1",
+                                  "inverse softplus", "mul+add"};
+    info.aten_refusal = aten_draw_refusal(tape, st.rng_chain);
+    for (size_t i = 0; i < st.segs.size() && info.aten_refusal.empty(); ++i) {
+      if (!st.segs[i].st.rng()) continue;
+      for (const TdxEpiStep& e : emitted[i]) {
+        if (aten_exact_step(e.op)) continue;
+        const uint32_t k = e.op & 0xffu;
+        info.aten_refusal = std::string("a draw feeds a ") + (k < 12 ? steps[k] : "?") +
+                            " step, which ATen's stream does not compute bit for bit";
+        break;
+      }
+    }
+    if (!info.aten_refusal.empty()) info.fusible = false;
   }
   return info;
 }

@@ -10,6 +10,7 @@
 #include <c10/util/SmallVector.h>
 
 #include <cstdint>
+#include <string>
 #include <vector>
 
 #include "planner.h"
@@ -148,6 +149,11 @@ bool build_fast(const StorageInfo& si, StorageTemplate& t, bool may_sync);
 // names its storage any more, nothing of it has been materialised, and the only ops that ever
 // touched it are its own writers and the cast.
 bool wide_observable(const Tape& tape, const Sym& sy);
+// RngStream::Aten's rule (planner_engine.cc aten_fusible).  Why ATen does not launch every draw of
+// `chain`, live or dead, as one 32-bit, trivially 1-D iterator ("": it does), and whether the kernels
+// compute epilogue step `op` on a draw bit for bit as ATen's CUDA op does.
+std::string aten_draw_refusal(const Tape& tape, const RngChain& chain);
+bool aten_exact_step(uint32_t op);
 // The position of argument `name` in the op's schema (size_t(-1): none).
 size_t find_arg(const TapeOp& op, const char* name);
 

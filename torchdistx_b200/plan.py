@@ -20,6 +20,10 @@ value (refused above ``max_embedded_bytes``).  Building a plan therefore MATERIA
 tensors on the recording (on their recorded device); it does so under a forked RNG state, so the
 caller's generators are left as they were, and it refuses programs that draw random numbers
 (embedding one sample would freeze it).
+
+``InitPlan.from_module(module, rng="aten")`` builds a plan whose draws take ATen's own CUDA stream, as
+``materialize_module(rng="aten")`` draws them (InitPlan/7): PyTorch's own bits and generator offsets,
+through ``materialize``, ``apply`` and ``init_sharded_module`` alike.
 """
 from __future__ import annotations
 
@@ -53,12 +57,27 @@ FORMAT_SINCOS = "torchdistx_b200.InitPlan/4"
 FORMAT_GATHER = "torchdistx_b200.InitPlan/5"
 # Plans with a band mask (a "band" segment, TDX_SRC_BAND: a causal-mask buffer) are version 6.
 FORMAT_BAND = "torchdistx_b200.InitPlan/6"
+# Plans built for ATen's own CUDA stream (``from_module(rng="aten")``: TDX_ALGO_ATEN draws, ATen's generator
+# offsets) are version 7, with a top-level ``"rng": "aten"``; each drawn segment records "aten_wide".
+FORMAT_ATEN = "torchdistx_b200.InitPlan/7"
+_FORMATS = (FORMAT_ATEN, FORMAT_BAND, FORMAT_GATHER, FORMAT_SINCOS, FORMAT_SSM, FORMAT, "torchdistx_b200.InitPlan/1")
 
 
 def offset_increment(numel: int) -> int:
     """Generator offset one RNG pass over `numel` elements consumes (planner_engine.cc assign_rng)."""
     blocks = (numel + 3) // 4
     return ((blocks + 3) // 4) * 4 + 4
+
+
+# `aten` below: the (multiprocessor count, max threads per multiprocessor) of the device an ``rng="aten"``
+# plan is built on.  ATen's launch of a draw, and so its grid stride S and its generator offset increment,
+# depend on them (``_C.aten_stream_policy``); None: the default stream.
+DeviceProps = Optional[Tuple[int, int]]
+
+
+def _aten_policy(numel: int, aten: Tuple[int, int]) -> Tuple[int, int]:
+    """(S, offset increment) of ATen's launch of one draw of `numel` elements on a device `aten`."""
+    return tuple(_C.aten_stream_policy(numel, aten[0], aten[1]))
 
 
 @dataclass
@@ -91,7 +110,9 @@ class PlanEntry:
     #  host-built tensor) "gather_bytes" (base64 of the source, in the entry's dtype),
     #  "gather_period", "gather_repeat" (its broadcast geometry, 0 / 0: a plain copy), and for "band"
     #  segments (a band mask of an [..., R, C] tensor) "band_rows", "band_cols", "band_lo", "band_hi"
-    #  and "band_in", "band_out" (the element bits inside and outside the band, as integers)}
+    #  and "band_in", "band_out" (the element bits inside and outside the band, as integers), and in an
+    #  ``rng="aten"`` plan, for "uniform" / "normal" segments, "aten_wide" (the draw ran on fp32 and is
+    #  rounded at the store: TDX_ALGO_ATEN_WIDE; such a plan lists every entry with a draw as segments)}
     segments: List[dict] = field(default_factory=list)
 
     def segment_list(self) -> List[dict]:
@@ -202,10 +223,12 @@ def narrowed(e: "PlanEntry", shard: Optional[Tuple[int, int]] = None, dim: Optio
         g["source"] in ("iota", "sincos", "gather", "band") for g in e.segment_list())
 
 
-def assign_pass_offsets(e: "PlanEntry", assigned: Dict[int, int], offset: int) -> Tuple[List[int], int]:
+def assign_pass_offsets(e: "PlanEntry", assigned: Dict[int, int], offset: int,
+                        aten: DeviceProps = None) -> Tuple[List[int], int]:
     """Philox offsets of the entry's RNG passes, and the generator offset after them.  Every pass on
     the chain takes its slice of the stream once per pass identity: a clone names its source's
-    passes again (same stream, nothing consumed)."""
+    passes again (same stream, nothing consumed).  `aten`: each pass, dead ones included, advances the
+    generator as ATen's launch of it does on that device."""
     ids = e.rng_ids if e.rng_ids else [None] * len(e.rng_numels)
     pass_offset = []
     for pid, n in zip(ids, e.rng_numels):
@@ -215,7 +238,7 @@ def assign_pass_offsets(e: "PlanEntry", assigned: Dict[int, int], offset: int) -
         pass_offset.append(offset)
         if pid is not None:
             assigned[pid] = offset
-        offset += offset_increment(n)
+        offset += _aten_policy(n, aten)[1] if aten else offset_increment(n)
     return pass_offset, offset
 
 
@@ -225,14 +248,17 @@ def gather_source(g: dict, dtype: torch.dtype) -> torch.Tensor:
 
 
 def entry_descriptors(e: "PlanEntry", base: int, begin: int, count: int, seed: int,
-                      pass_offset: List[int], gather_src=None, window: Optional[Tuple[int, int]] = None) -> list:
+                      pass_offset: List[int], gather_src=None, window: Optional[Tuple[int, int]] = None,
+                      aten: DeviceProps = None) -> list:
     """The C-ABI descriptors that write elements [begin, begin + count) of an entry into a buffer
     whose first byte is at address `base` (plain data in, ``TdxInitDesc`` out: no device needed).
     `gather_src(segment)` gives the device address of a "gather" segment's source (default 0: the
     source is not on a device; a host restatement reads it from the segment).  `window` = (W, P): the
     part is count / W runs of W elements, P apart, from `begin` (a Shard(d >= 1) block): per segment,
     the partial runs at its ends are plain descriptors, its whole runs one windowed descriptor (RNG)
-    or one fill (constants) -- what the planner emits (planner_engine.cc emit_window)."""
+    or one fill (constants) -- what the planner emits (planner_engine.cc emit_window).  `aten`: the draws
+    take ATen's stream on that device (TDX_ALGO_ATEN / TDX_ALGO_ATEN_WIDE, ``fill_bits[1]`` = its grid
+    stride S, and a window in ``fill_bits[0]`` as ``W | P << 32``)."""
     dtype = _DTYPES[e.dtype]
     isz = torch.empty((), dtype=dtype).element_size()
     if window is not None:
@@ -253,17 +279,21 @@ def entry_descriptors(e: "PlanEntry", base: int, begin: int, count: int, seed: i
                     continue
                 if (lo, hi) == (rb, rb + W):  # runs [o, last) lie inside the segment
                     last = min(count // W, (g["end"] - begin - W) // P + 1)
-                    (d,) = entry_descriptors(PlanEntry(**one), base + o * W * isz, rb, W, seed, pass_offset, gather_src)
+                    (d,) = entry_descriptors(PlanEntry(**one), base + o * W * isz, rb, W, seed, pass_offset, gather_src,
+                                             aten=aten)
                     if last - o > 1:
                         d.elem_count = (last - o) * W  # (a constant's whole runs are contiguous: one fill)
                         if g["source"] != "const":
                             d.reserved |= _cabi.TDX_FLAG_WINDOW
-                            d.fill_bits[0], d.fill_bits[1] = W, P
+                            if aten:  # (fill_bits[1] is ATen's grid stride)
+                                d.fill_bits[0] = W | P << 32
+                            else:
+                                d.fill_bits[0], d.fill_bits[1] = W, P
                     descs.append(d)
                     o = last
                 else:
                     descs += entry_descriptors(PlanEntry(**one), base + (o * W + lo - rb) * isz, lo, hi - lo,
-                                               seed, pass_offset, gather_src)
+                                               seed, pass_offset, gather_src, aten=aten)
                     o += 1
         return descs
     descs = []
@@ -299,26 +329,45 @@ def entry_descriptors(e: "PlanEntry", base: int, begin: int, count: int, seed: i
                 band_rows=g["band_rows"], band_cols=g["band_cols"], band_lo=g["band_lo"], band_hi=g["band_hi"],
                 band_in=g["band_in"], band_out=g["band_out"]))
         else:
+            if aten:  # (the draw's dtype, whether or not the fp32 tensor is observable: it changes bits)
+                algo = _cabi.TDX_ALGO_ATEN_WIDE if g["aten_wide"] else _cabi.TDX_ALGO_ATEN
+                stride = _aten_policy(e.rng_numels[g["rng_pass"]], aten)[0]
+            else:
+                algo, stride = (_cabi.TDX_ALGO_WIDE32 if g["wide"] else 0), 0
             descs.append(_cabi.make_desc(
                 dst, dtype=_TDX_DTYPE[dtype],
                 src=_cabi.TDX_SRC_UNIFORM if g["source"] == "uniform" else _cabi.TDX_SRC_NORMAL,
                 elem_begin=lo - g["origin"], elem_count=hi - lo, seed=seed,
                 offset=pass_offset[g["rng_pass"]], p0=g["p0"], p1=g["p1"],
-                epi=g["epilogue"], algo=_cabi.TDX_ALGO_WIDE32 if g["wide"] else 0,
+                epi=g["epilogue"], algo=algo, aten_stride=stride,
                 flags=_cabi.TDX_FLAG_SRC_NOROUND if g["src_noround"] else 0))
     return descs
 
 
 class InitPlan:
-    def __init__(self, entries: List[PlanEntry]):
+    def __init__(self, entries: List[PlanEntry], rng: str = "fused"):
+        if rng not in ("fused", "aten"):
+            raise ValueError(f'rng must be "fused" or "aten", got "{rng}"')
         self.entries = entries
+        self.rng = rng  # the stream the plan's draws take: materialize_module's `rng`
 
     # ------------------------------------------------------------------------------------- build
     @classmethod
-    def from_module(cls, module: Module, max_embedded_bytes: int = 1 << 20) -> "InitPlan":
+    def from_module(cls, module: Module, max_embedded_bytes: int = 1 << 20, rng: str = "fused") -> "InitPlan":
         """Builds the plan of a module created by ``deferred_init``.  Traversal order is the one
-        ``materialize_module`` uses (children first, then own parameters, then own buffers)."""
+        ``materialize_module`` uses (children first, then own parameters, then own buffers).
+
+        `rng="aten"`: the plan's draws take ATen's own CUDA stream, as ``materialize_module(rng="aten")``
+        draws them: after the same ``torch.manual_seed`` its tensors and the generator's offset are
+        eager CUDA's.  Each drawn segment records whether the draw ran on fp32 (rounded at the store);
+        the grid stride S of each draw is not recorded, it is the materialising device's.  A tensor
+        whose random program ATen's stream cannot take (a draw through a non-contiguous view, one that
+        needs 64-bit indexing, a step the kernels do not compute as ATen does) raises ``ValueError``:
+        ``materialize_module`` replays such a tensor through ATen, a plan cannot."""
         from .deferred_init import materialize_tensor
+
+        if rng not in ("fused", "aten"):
+            raise ValueError(f'rng must be "fused" or "aten", got "{rng}"')
 
         entries: List[PlanEntry] = []
         seen: Dict[int, str] = {}
@@ -336,7 +385,10 @@ class InitPlan:
                         entries.append(PlanEntry(name, kind, list(t.shape), _DTYPE_NAMES[t.dtype], "alias", alias_of=seen[id(t)]))
                         continue
                     seen[id(t)] = name
-                    info = dict(_C.plan_info(t))
+                    info = dict(_C.plan_info(t, rng))
+                    if info.get("aten_refusal"):
+                        raise ValueError(f"'{name}' has a random initialisation program ATen's stream cannot take "
+                                         f"({info['aten_refusal']}); an rng=\"aten\" plan cannot hold it")
                     if info["source"] in ("const", "uniform", "normal", "uninit", "iota", "sincos", "gather", "band") \
                             and info["fusible"]:
                         segs = [dict(begin=g["begin"], end=g["end"], origin=g["origin"], source=g["source"],
@@ -358,14 +410,18 @@ class InitPlan:
                             if g["source"] == "band":
                                 for k in ("band_rows", "band_cols", "band_lo", "band_hi", "band_in", "band_out"):
                                     s[k] = int(g[k])
-                        # (broadcast, table and band geometry, and gather sources, only live in the segment list)
-                        geometry = any("iota_period" in s or s["source"] in ("sincos", "gather", "band") for s in segs)
+                            if rng == "aten" and g["source"] in ("uniform", "normal"):
+                                s["aten_wide"] = bool(g["aten_wide"])
+                        # (broadcast, table and band geometry, gather sources and the draw dtype of ATen's
+                        # stream only live in the segment list)
+                        only_listed = any("iota_period" in s or "aten_wide" in s or s["source"] in ("sincos", "gather", "band")
+                                          for s in segs)
                         entries.append(PlanEntry(
                             name, kind, list(info["sizes"]), info["dtype"], info["source"], info["p0"], info["p1"],
                             [tuple(e) for e in info["epilogue"]],
                             base64.b64encode(info["const_bytes"]).decode(), "", list(info["rng_numels"]),
                             bool(info["requires_grad"]), None, bool(info["wide"]), bool(info["src_noround"]),
-                            [int(i) for i in info["rng_op_ids"]], segs if len(segs) > 1 or geometry else []))
+                            [int(i) for i in info["rng_op_ids"]], segs if len(segs) > 1 or only_listed else []))
                         continue
                     # not fusible (or already real): evaluate now and store by value -- under a forked
                     # RNG state, and never a program that draws random numbers (one frozen sample)
@@ -400,14 +456,17 @@ class InitPlan:
                                              requires_grad=bool(real.requires_grad)))
 
         visit(module, "")
-        return cls(entries)
+        return cls(entries, rng)
 
     # --------------------------------------------------------------------------------------- io
     def save(self, path: str) -> None:
         with open(path, "w") as f:
-            fmt = (FORMAT_BAND if self.uses_band() else FORMAT_GATHER if self.uses_gather()
-                   else FORMAT_SINCOS if self.uses_sincos() else FORMAT_SSM if self.uses_ssm() else FORMAT)
-            json.dump({"format": fmt, "entries": [e.__dict__ for e in self.entries]}, f)
+            if self.rng == "aten":
+                doc = {"format": FORMAT_ATEN, "rng": "aten"}
+            else:
+                doc = {"format": FORMAT_BAND if self.uses_band() else FORMAT_GATHER if self.uses_gather()
+                       else FORMAT_SINCOS if self.uses_sincos() else FORMAT_SSM if self.uses_ssm() else FORMAT}
+            json.dump({**doc, "entries": [e.__dict__ for e in self.entries]}, f)
 
     def uses_band(self) -> bool:
         """Does the plan hold a band mask (written as InitPlan/6)?"""
@@ -435,15 +494,18 @@ class InitPlan:
     def load(cls, path: str) -> "InitPlan":
         with open(path) as f:
             doc = json.load(f)
-        if doc.get("format") not in (FORMAT_BAND, FORMAT_GATHER, FORMAT_SINCOS, FORMAT_SSM, FORMAT, "torchdistx_b200.InitPlan/1"):
+        if doc.get("format") not in _FORMATS:
             raise ValueError(f"{path}: not an {FORMAT} file")
+        rng = doc.get("rng", "fused")
+        if (doc["format"] == FORMAT_ATEN) != (rng == "aten"):
+            raise ValueError(f"{path}: a {doc['format']} file with rng {rng!r}")
         entries = []
         for d in doc["entries"]:
             d["epilogue"] = [tuple(e) for e in d.get("epilogue", [])]
             for g in d.get("segments", []):
                 g["epilogue"] = [tuple(e) for e in g.get("epilogue", [])]
             entries.append(PlanEntry(**d))
-        return cls(entries)
+        return cls(entries, rng)
 
     @property
     def num_params(self) -> int:
@@ -466,7 +528,8 @@ class InitPlan:
         return chunk_steps(e, shard, 0 if placements is None else placements.get(e.name))
 
     def descriptors(self, seed: int, offset: int, shard: Optional[Tuple[int, int]] = None, gather_src=None,
-                    placements: Optional[Dict[str, Optional[int]]] = None, blocks: Optional[Dict[str, Steps]] = None):
+                    placements: Optional[Dict[str, Optional[int]]] = None, blocks: Optional[Dict[str, Steps]] = None,
+                    device_props: DeviceProps = None):
         """The plan as the C ABI sees it, without a device: ``([(entry, sizes, descs)], offset after)``
         for the tensors :meth:`materialize` would build from generator state ``(seed, offset)`` on
         this rank.  ``descs`` address each tensor from byte 0 (``dst`` = byte offset inside it); value
@@ -485,7 +548,13 @@ class InitPlan:
         layout whose local blocks are rows of dim 0 times at most one range of another dimension, such
         as FSDP2 over tensor parallelism on a 2-D mesh -- each listed entry is its block
         (:func:`block_ranges`), every other entry is whole; not combined with `shard` / `placements`.
-        Entries built whole and narrowed are listed whole, as above."""
+        Entries built whole and narrowed are listed whole, as above.
+
+        `device_props` = (multiprocessor count, max threads per multiprocessor) of the device that will
+        run the table: required for an ``rng="aten"`` plan, whose draws take ATen's launch on that device
+        (each drawn descriptor carries its grid stride S in ``fill_bits[1]``, and each pass advances
+        the generator by ATen's increment); ignored otherwise."""
+        aten = self._aten_props(device_props)
         assigned: Dict[int, int] = {}
         table = []
         for e in self.entries:
@@ -496,10 +565,19 @@ class InitPlan:
             if narrowed(e, steps=steps):
                 steps = []
             begin, count, sizes = shard_range(e, steps=steps)
-            pass_offset, offset = assign_pass_offsets(e, assigned, offset)
+            pass_offset, offset = assign_pass_offsets(e, assigned, offset, aten)
             table.append((e, sizes, entry_descriptors(e, 0, begin, count, seed, pass_offset, gather_src,
-                                                      shard_window(e, steps=steps))))
+                                                      shard_window(e, steps=steps), aten)))
         return table, offset
+
+    def _aten_props(self, device_props: DeviceProps) -> DeviceProps:
+        if self.rng != "aten":
+            return None
+        if device_props is None:
+            raise ValueError('an rng="aten" plan needs the device\'s (multiprocessor count, max threads per '
+                             'multiprocessor) as `device_props`: its draws take ATen\'s launch on that device')
+        sm, tps = (int(x) for x in device_props)
+        return sm, tps
 
     # ------------------------------------------------------------------------------ materialise
     def materialize(self, device="cuda", shard: Optional[Tuple[int, int]] = None,
@@ -522,6 +600,9 @@ class InitPlan:
 
         `blocks`: each listed entry is its block of chunk steps, every other entry whole, as for
         :meth:`descriptors` (the FSDP x TP hand-off of :func:`init_sharded_module`).
+
+        An ``rng="aten"`` plan draws from ATen's stream as laid out for `device` (its multiprocessor
+        count and threads per multiprocessor), under every layout above.
         """
         device = torch.device(device)
         if device.type != "cuda":
@@ -530,6 +611,10 @@ class InitPlan:
             device = torch.device("cuda", torch.cuda.current_device())
         gen = generator or torch.cuda.default_generators[device.index]
         seed, offset = gen.initial_seed(), gen.get_offset()
+        aten = None
+        if self.rng == "aten":
+            props = torch.cuda.get_device_properties(device)
+            aten = props.multi_processor_count, props.max_threads_per_multi_processor
         out: Dict[str, torch.Tensor] = {}
         descs = []
         staged: List[torch.Tensor] = []  # gather sources on the device: alive until the launch is queued
@@ -567,9 +652,9 @@ class InitPlan:
                     t = target
                 else:
                     t = torch.empty(sizes, dtype=dtype, device=device)
-                pass_offset, offset = assign_pass_offsets(e, assigned, offset)
+                pass_offset, offset = assign_pass_offsets(e, assigned, offset, aten)
                 descs += entry_descriptors(e, t.data_ptr(), begin, count, seed, pass_offset, gather_src,
-                                           shard_window(e, steps=steps))
+                                           shard_window(e, steps=steps), aten)
                 out[e.name] = t if target is not None else _wrap(t, e)
             if descs:
                 ws_bytes = _cabi.prepare(descs)  # exactly what this table needs (not the ~1.6 MB upper bound)
