@@ -358,12 +358,16 @@ struct NanAcc<__half> {
 // function, hence the same bits), the parameters that identify a table, and whether some k needs the
 // exact out-of-line path (the normal's k == 0 tail).
 // Two descriptors of one table-kernel family share a table iff their generator parameters and
-// epilogues are equal (dtype, source and "has an epilogue" are the family's).
+// epilogues are equal (dtype, source and "has an epilogue" are the family's).  Equal as bit patterns:
+// +0 and -0 compare equal as numbers but give tables of opposite signed zeros (normal_(+0, 0) against
+// normal_(-0, 0), uniform_(-0, -0) against uniform_(-0, +0), mul_(0) against mul_(-0)).
 __device__ __forceinline__ bool same_table(const TdxInitDesc& a, const TdxInitDesc& b) {
-  bool same = a.p0 == b.p0 && a.p1 == b.p1 && a.n_epi == b.n_epi && a.reserved == b.reserved;
+  bool same = __double_as_longlong(a.p0) == __double_as_longlong(b.p0) &&
+              __double_as_longlong(a.p1) == __double_as_longlong(b.p1) && a.n_epi == b.n_epi && a.reserved == b.reserved;
   for (int i = 0; i < TDX_MAX_EPI; ++i)
     if (i < a.n_epi)
-      same = same && a.epi[i].op == b.epi[i].op && a.epi[i].a == b.epi[i].a && a.epi[i].b == b.epi[i].b;
+      same = same && a.epi[i].op == b.epi[i].op && __float_as_uint(a.epi[i].a) == __float_as_uint(b.epi[i].a) &&
+             __float_as_uint(a.epi[i].b) == __float_as_uint(b.epi[i].b);
   return same;
 }
 
@@ -375,10 +379,13 @@ struct TabNormal {
   using Gen = GenNormalICDF16<Out, EPI>;
   using Params = typename Gen::Params;
   static constexpr bool kHasTail = true;
-  // The grid x = k/32768 - 1 is symmetric about k = 32768 and, with mean == +0 and no epilogue, so is
-  // the value (fma(q, -x, +0) == -fma(q, x, +0), rounding included): the upper half of the table is
-  // the lower half with the sign bit flipped -- half the evaluations per table build.
-  __device__ static __forceinline__ bool mirrored(const Params& p) { return !EPI && __float_as_uint(p.mean) == 0u; }
+  // The grid x = k/32768 - 1 is symmetric about k = 32768 and, with mean == +0, std != 0 and no
+  // epilogue, so is the value (fma(q, -x, +0) == -fma(q, x, +0), rounding included): the upper half of
+  // the table is the lower half with the sign bit flipped -- half the evaluations per table build.
+  // With std == +-0 every q x is an exact zero and +-0 + +0 is +0 for both signs of x: no mirror.
+  __device__ static __forceinline__ bool mirrored(const Params& p) {
+    return !EPI && __float_as_uint(p.mean) == 0u && p.std != 0.f;
+  }
   __device__ static __forceinline__ float value(const Params& p, float magic) {
     float t;
     const float v = Gen::element(p, magic, t);  // k == 0: +-inf or NaN (lg2(0) = -inf)
