@@ -229,6 +229,17 @@ typedef struct TdxInitDesc {
   TdxEpiStep epi[TDX_MAX_EPI];
 } TdxInitDesc;
 
+/*
+ * A table may mix any descriptors: the library routes each to a kernel family (80 of them: the
+ * generators by dtype, algo, epilogue class, window and stream; the table kernels; the deterministic
+ * sources) and issues one launch per family the table uses.  One plan header holds 47 families;
+ * tdx_init_launch / tdx_init_prepare + tdx_init_submit lay a table that spans more out as consecutive
+ * plans in one workspace (each with its own header and work counters) and launch them in order on the
+ * stream, so any table is taken whole.  tdx_plan_upload keeps to one plan: a table of more than 47
+ * families is refused there (TDX_E_BADARG).  Which kernel a descriptor runs in is decided over the whole
+ * table, not per plan, so the split changes no bit.
+ */
+
 /* Bytes of device workspace tdx_init_launch() needs for `n` descriptors. */
 TDX_C_API size_t tdx_init_workspace_bytes(int n);
 
@@ -262,6 +273,7 @@ TDX_C_API int tdx_init_submit(void* workspace, size_t workspace_bytes, void* str
  * kernels (the work counters in the workspace are uploaded as zero and every
  * kernel puts its own back to zero when its last CTA leaves, so there is no
  * memset between launches; one plan must not run on two streams at once).
+ * One plan: at most 47 kernel families (see above), else TDX_E_BADARG.
  */
 typedef struct TdxPlan {
   uint64_t opaque[512]; /* host-side copy of the plan header; owned by the caller */

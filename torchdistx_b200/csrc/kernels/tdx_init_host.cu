@@ -154,10 +154,10 @@ uint64_t tiles_of(const TdxInitDesc& d, int tile_vecs) {
   return (nvec + tile_vecs - 1) / tile_vecs;
 }
 
-// Device-resident plan header.  Lives at the start of the caller's workspace.
+// Device-resident plan header.  Lives at the start of its plan image in the caller's workspace.
 struct PlanGroup {
   unsigned long long total_tiles;
-  unsigned long long prefix_off;  // byte offsets from the workspace base
+  unsigned long long prefix_off;  // byte offsets from the start of the plan image
   unsigned long long desc_off;
   uint32_t n_desc;
   uint32_t family;
@@ -176,14 +176,22 @@ struct PlanHeader {
   unsigned int done[64];
   // One per kernel family the plan uses -- a handful.  47 is what fits the 4 KiB TdxPlan
   // (static_assert in tdx_plan_upload: 520 + 47 * 72 + 128 <= 4096), fewer than there are families;
-  // build_plan refuses a submission that spans more (kMaxGroups).  Adding a field to PlanGroup or
-  // PlanHeader means lowering this bound.
+  // build_plan lays a submission that spans more out as consecutive plan images (kMaxGroups groups
+  // each).  Adding a field to PlanGroup or PlanHeader means lowering this bound.
   PlanGroup groups[47];
   TdxInitDesc one;  // the plan's descriptor if it has exactly one (GroupArgs::one)
 };
 constexpr uint32_t kPlanMagic = 0x58445431u;  // "TDX1"
 constexpr uint32_t kMaxGroups = sizeof(PlanHeader::groups) / sizeof(PlanGroup);
 static_assert(kMaxGroups <= 64, "counter slots (one per group of a plan)");
+// Plan images start on this boundary of the workspace (a descriptor table is 128-byte aligned).
+constexpr size_t kImageAlign = 256;
+
+// A prepared submission: one plan image per kMaxGroups kernel families, back to back in one workspace.
+struct PlanSet {
+  std::vector<PlanHeader> hdrs;
+  std::vector<size_t> base;  // byte offset of each image (and its header) in the workspace
+};
 
 // Work list of the table kernel: at most kMaxListChunks "large" grabs (the grab cap grows with the
 // launch so that this holds), a guided tail, and one partial grab per descriptor.
@@ -200,9 +208,11 @@ size_t lut_family_count() {
 }
 size_t plan_bytes(int n) {
   const size_t families_n = families().size();
-  // header + per-family prefix arrays (n + #families entries worst case) + descriptors + one work
-  // list per table family (each at most kMaxListChunks + kMaxListTail grabs plus one per descriptor)
-  return sizeof(PlanHeader) + (static_cast<size_t>(n) + families_n) * sizeof(unsigned long long) +
+  const size_t images = (families_n + kMaxGroups - 1) / kMaxGroups;
+  // one header per image (and its alignment) + per-family prefix arrays (n + #families entries worst
+  // case) + descriptors + one work list per table family (each at most kMaxListChunks + kMaxListTail
+  // grabs plus one per descriptor)
+  return images * (sizeof(PlanHeader) + kImageAlign) + (static_cast<size_t>(n) + families_n) * sizeof(unsigned long long) +
          static_cast<size_t>(n) * sizeof(TdxInitDesc) +
          (lut_family_count() * (kMaxListChunks + kMaxListTail) + static_cast<size_t>(n)) * sizeof(uint4) +
          lut_family_count() * kMaxListCtas * sizeof(uint32_t) +
@@ -243,10 +253,13 @@ DeviceInfo* device_info() {
   return &infos[dev];
 }
 
-// Builds the host image of the plan.  Returns 0 or an error code.
+// Builds the host image of the plan: one plan image per kMaxGroups kernel families, each with its own
+// header, work counters and offsets counted from its own start.  Routing (table or direct kernel,
+// riders) is decided over the whole table first, so a table that spans several images runs the
+// kernels it would run in one.  Returns 0 or an error code.
 // `img` is scratch that only grows (zero-filling 1.6 MB per call would cost more host time than the
 // planning of a small module); `used` = bytes of the image to copy to the device.
-int build_plan(const TdxInitDesc* descs, int n, std::vector<unsigned char>& img, PlanHeader& hdr, size_t& used) {
+int build_plan(const TdxInitDesc* descs, int n, std::vector<unsigned char>& img, PlanSet& plans, size_t& used) {
   if (n < 0 || (n > 0 && descs == nullptr)) return fail(TDX_E_BADARG, "descs == NULL or n < 0");
   const std::vector<Family>& F = families();
   if (F.empty()) return fail(TDX_E_BADARG, "internal: two kernel families overlap (see stderr)");
@@ -382,6 +395,9 @@ int build_plan(const TdxInitDesc* descs, int n, std::vector<unsigned char>& img,
         }
     }
   }
+  plans.hdrs.clear();
+  plans.base.clear();
+  PlanHeader hdr;
   memset(&hdr, 0, sizeof(hdr));
   hdr.magic = kPlanMagic;
   if (img.size() < plan_bytes(n)) img.resize(plan_bytes(n));
@@ -390,21 +406,32 @@ int build_plan(const TdxInitDesc* descs, int n, std::vector<unsigned char>& img,
   std::vector<int> order;
   thread_local std::vector<uint32_t> seg_fill;
   order.reserve(static_cast<size_t>(n));
-  size_t off = (sizeof(PlanHeader) + 15) & ~static_cast<size_t>(15);
+  const size_t hdr_end = (sizeof(PlanHeader) + 15) & ~static_cast<size_t>(15);
+  size_t start = 0, off = hdr_end;  // the current image's offset in the workspace; `off` counts from it
+  unsigned char* image = img.data();
   for (int f = 0; f < nf; ++f) {
     if (!per_family[f]) continue;
-    if (hdr.n_groups == kMaxGroups) return fail(TDX_E_BADARG, "the descriptors span more kernel families than a plan holds");
+    if (hdr.n_groups == kMaxGroups) {  // this image is full: the next family opens another
+      memcpy(image, &hdr, sizeof(hdr));
+      plans.hdrs.push_back(hdr);
+      plans.base.push_back(start);
+      start = (start + off + kImageAlign - 1) & ~(kImageAlign - 1);
+      image = img.data() + start;
+      off = hdr_end;
+      memset(&hdr, 0, sizeof(hdr));
+      hdr.magic = kPlanMagic;
+    }
     PlanGroup& G = hdr.groups[hdr.n_groups++];
     G.family = f;
     G.n_desc = per_family[f];
     // (8-byte prefix sums: the table kernel's segment table before this group ends on a 4-byte boundary)
     off = (off + 15) & ~static_cast<size_t>(15);
     G.prefix_off = off;
-    auto* prefix = reinterpret_cast<unsigned long long*>(img.data() + off);
+    auto* prefix = reinterpret_cast<unsigned long long*>(image + off);
     off += (static_cast<size_t>(G.n_desc) + 1) * sizeof(unsigned long long);
     off = (off + 127) & ~static_cast<size_t>(127);  // (a descriptor = one cache line: lut_prefetch_desc)
     G.desc_off = off;
-    auto* out = reinterpret_cast<TdxInitDesc*>(img.data() + off);
+    auto* out = reinterpret_cast<TdxInitDesc*>(image + off);
     off += static_cast<size_t>(G.n_desc) * sizeof(TdxInitDesc);
     unsigned long long acc = 0;
     uint32_t k = 0;
@@ -436,7 +463,9 @@ int build_plan(const TdxInitDesc* descs, int n, std::vector<unsigned char>& img,
       }
       prefix[k] = acc;
       out[k] = descs[i];
-      if (n == 1) hdr.one = descs[i];
+      // (an image of one group of one descriptor launches it inline: the last image of a split table
+      // can be one even when the table is not)
+      if (G.n_desc == 1) hdr.one = descs[i];
       acc += tiles_of(descs[i], F[f].tile_vecs);
       ++k;
     }
@@ -454,7 +483,7 @@ int build_plan(const TdxInitDesc* descs, int n, std::vector<unsigned char>& img,
       // costs throughput.  Small launches (fewer than 16 tiles per CTA) are all tail.
       off = (off + 15) & ~static_cast<size_t>(15);
       G.chunk_off = off;
-      auto* list = reinterpret_cast<uint4*>(img.data() + off);
+      auto* list = reinterpret_cast<uint4*>(image + off);
       const unsigned long long ctas = static_cast<unsigned long long>(std::max(sm_count, 1));
       const unsigned long long cap =
           std::max<unsigned long long>(kLutMaxGrabBytes / (F[f].tile_vecs * 16ull), (acc + kMaxListChunks - 1) / kMaxListChunks);
@@ -474,7 +503,7 @@ int build_plan(const TdxInitDesc* descs, int n, std::vector<unsigned char>& img,
           } else {
             sz = std::min(std::min(std::max(remaining / (2ull * ctas), 1ull), cap), nt - t);
           }
-          if (off + (static_cast<size_t>(nc) + 1) * sizeof(uint4) > img.size())
+          if (start + off + (static_cast<size_t>(nc) + 1) * sizeof(uint4) > img.size())
             return fail(TDX_E_WORKSPACE, "internal: work list exceeds its bound");
           list[nc++] = make_uint4(di, static_cast<uint32_t>(sz), static_cast<uint32_t>(t),
                                   static_cast<uint32_t>(t >> 32));
@@ -496,16 +525,18 @@ int build_plan(const TdxInitDesc* descs, int n, std::vector<unsigned char>& img,
       G.list_ctas = static_cast<uint32_t>(ctas);
       G.seg_off_off = off;
       if (static_tiles && cta == ctas) {
-        if (off + (static_cast<size_t>(ctas) + 1) * sizeof(uint32_t) > img.size())
+        if (start + off + (static_cast<size_t>(ctas) + 1) * sizeof(uint32_t) > img.size())
           return fail(TDX_E_WORKSPACE, "internal: segment table exceeds its bound");
-        memcpy(img.data() + off, seg_fill.data(), (static_cast<size_t>(ctas) + 1) * sizeof(uint32_t));
+        memcpy(image + off, seg_fill.data(), (static_cast<size_t>(ctas) + 1) * sizeof(uint32_t));
         G.n_static = seg_fill[ctas];
         off += (static_cast<size_t>(ctas) + 1) * sizeof(uint32_t);
       }
     }
   }
-  memcpy(img.data(), &hdr, sizeof(hdr));
-  used = off;
+  memcpy(image, &hdr, sizeof(hdr));
+  plans.hdrs.push_back(hdr);
+  plans.base.push_back(start);
+  used = start + off;
   return 0;
 }
 
@@ -554,12 +585,12 @@ int stage(const void* src, size_t bytes, cudaStream_t stream, void* dst_device, 
   return 0;
 }
 
-int launch_groups(const PlanHeader& hdr, void* workspace, cudaStream_t stream) {
+// Launches the groups of one plan image whose device copy starts at `image`; adds them to `launches`.
+int launch_groups(const PlanHeader& hdr, void* image, cudaStream_t stream, int& launches) {
   DeviceInfo* info = device_info();
   if (!info) return fail(TDX_E_NODEVICE, "no CUDA device / occupancy query failed");
-  auto* base = static_cast<unsigned char*>(workspace);
+  auto* base = static_cast<unsigned char*>(image);
   auto* dev_hdr = reinterpret_cast<PlanHeader*>(base);
-  int launches = 0;
   for (uint32_t gi = 0; gi < hdr.n_groups; ++gi) {
     const PlanGroup& G = hdr.groups[gi];
     if (G.total_tiles == 0) continue;
@@ -612,7 +643,6 @@ int launch_groups(const PlanHeader& hdr, void* workspace, cudaStream_t stream) {
     if (e != cudaSuccess) return cuda_fail(e, F.name);
     ++launches;
   }
-  g_last_launches = launches;
   return 0;
 }
 
@@ -626,11 +656,14 @@ TDX_C_API int tdx_plan_upload(const TdxInitDesc* descs, int n, void* workspace,
                               size_t workspace_bytes, void* stream, TdxPlan* plan) {
   static_assert(sizeof(tdx::PlanHeader) <= sizeof(TdxPlan), "TdxPlan too small");
   thread_local std::vector<unsigned char> img;
-  tdx::PlanHeader hdr;
+  thread_local tdx::PlanSet plans;
   if (plan == nullptr) return tdx::fail(TDX_E_BADARG, "plan == NULL");
   size_t used = 0;
-  if (int rc = tdx::build_plan(descs, n, img, hdr, used)) return rc;
-  memcpy(plan, &hdr, sizeof(hdr));
+  if (int rc = tdx::build_plan(descs, n, img, plans, used)) return rc;
+  if (plans.hdrs.size() != 1)
+    return tdx::fail(TDX_E_BADARG, "tdx_plan_upload: the descriptors span more kernel families than one plan holds "
+                                   "(47); tdx_init_launch takes them");
+  memcpy(plan, &plans.hdrs[0], sizeof(tdx::PlanHeader));
   if (workspace == nullptr || workspace_bytes < used)
     return tdx::fail(TDX_E_WORKSPACE, "workspace too small (see tdx_init_workspace_bytes)");
   tdx::g_last_upload_bytes = used;
@@ -649,13 +682,16 @@ TDX_C_API int tdx_plan_launch(const TdxPlan* plan, void* workspace, void* stream
   tdx::PlanHeader hdr;
   memcpy(&hdr, plan, sizeof(hdr));
   if (hdr.magic != tdx::kPlanMagic) return tdx::fail(TDX_E_BADARG, "plan was not produced by tdx_plan_upload");
-  return tdx::launch_groups(hdr, workspace, static_cast<cudaStream_t>(stream));
+  int launches = 0;
+  if (int rc = tdx::launch_groups(hdr, workspace, static_cast<cudaStream_t>(stream), launches)) return rc;
+  tdx::g_last_launches = launches;
+  return 0;
 }
 
 // The host image of the plan tdx_init_prepare() built on this thread, waiting for tdx_init_submit().
 namespace tdx {
 thread_local std::vector<unsigned char> g_prepared_img;
-thread_local PlanHeader g_prepared_hdr;
+thread_local PlanSet g_prepared_plans;
 thread_local size_t g_prepared_used = 0;
 thread_local bool g_prepared = false;
 }  // namespace tdx
@@ -663,8 +699,8 @@ thread_local bool g_prepared = false;
 TDX_C_API int tdx_init_prepare(const TdxInitDesc* descs, int n, size_t* workspace_bytes) {
   tdx::g_prepared = false;
   if (workspace_bytes == nullptr) return tdx::fail(TDX_E_BADARG, "workspace_bytes == NULL");
-  if (int rc = tdx::build_plan(descs, n, tdx::g_prepared_img, tdx::g_prepared_hdr, tdx::g_prepared_used)) return rc;
-  *workspace_bytes = tdx::g_prepared_hdr.n_groups ? tdx::g_prepared_used : 0;
+  if (int rc = tdx::build_plan(descs, n, tdx::g_prepared_img, tdx::g_prepared_plans, tdx::g_prepared_used)) return rc;
+  *workspace_bytes = tdx::g_prepared_plans.hdrs[0].n_groups ? tdx::g_prepared_used : 0;
   tdx::g_prepared = true;
   return 0;
 }
@@ -672,8 +708,8 @@ TDX_C_API int tdx_init_prepare(const TdxInitDesc* descs, int n, size_t* workspac
 TDX_C_API int tdx_init_submit(void* workspace, size_t workspace_bytes, void* stream) {
   if (!tdx::g_prepared) return tdx::fail(TDX_E_BADARG, "tdx_init_submit without tdx_init_prepare on this thread");
   tdx::g_prepared = false;
-  const tdx::PlanHeader& hdr = tdx::g_prepared_hdr;
-  if (hdr.n_groups == 0) {
+  const tdx::PlanSet& plans = tdx::g_prepared_plans;
+  if (plans.hdrs[0].n_groups == 0) {
     tdx::g_last_launches = 0;
     return 0;
   }
@@ -686,7 +722,13 @@ TDX_C_API int tdx_init_submit(void* workspace, size_t workspace_bytes, void* str
   void* pinned = nullptr;
   if (int rc = tdx::stage(tdx::g_prepared_img.data(), used, static_cast<cudaStream_t>(stream), workspace, &pinned))
     return rc;
-  return tdx::launch_groups(hdr, workspace, static_cast<cudaStream_t>(stream));
+  int launches = 0;
+  for (size_t p = 0; p < plans.hdrs.size(); ++p)
+    if (int rc = tdx::launch_groups(plans.hdrs[p], static_cast<unsigned char*>(workspace) + plans.base[p],
+                                    static_cast<cudaStream_t>(stream), launches))
+      return rc;
+  tdx::g_last_launches = launches;
+  return 0;
 }
 
 TDX_C_API int tdx_init_launch(const TdxInitDesc* descs, int n, void* workspace,
