@@ -282,6 +282,61 @@ TDX_C_API int tdx_plan_upload(const TdxInitDesc* descs, int n, void* workspace,
                               size_t workspace_bytes, void* stream, TdxPlan* plan);
 TDX_C_API int tdx_plan_launch(const TdxPlan* plan, void* workspace, void* stream);
 
+/*
+ * Host destinations (CPU-offloaded shards: FSDP2's CPUOffloadPolicy, FSDP1's offload_params).
+ * tdx_init_submit_host runs a table whose `dst` addresses are all host memory, pinned or pageable, in
+ * passes through a device staging buffer the caller owns (`staging`: device memory, 16-byte aligned,
+ * untouched until the stream has run the call's work).  Each pass:
+ *   1. places pieces of descriptors in the staging buffer -- a piece is the local elements [l0, l1) of
+ *      one descriptor, kept at its destination's address mod 16, so the kernels take the vector/element
+ *      split they take at the real address;
+ *   2. lays the pass's table out as tdx_init_prepare would, carves its plan workspace from the head of
+ *      `staging` and launches it on `stream`;
+ *   3. enqueues one cudaMemcpyAsync device-to-host per piece on `stream` (local element l of a descriptor
+ *      is at dst + l * itemsize: a piece is one contiguous copy).
+ * Stream order is the only synchronisation: the next pass's launch runs after the previous pass's copies
+ * have read the buffer.  The host does not block for pinned destinations; a pageable one makes its copy
+ * synchronous (CUDA's rule for pageable memory).  The values depend only on (seed, offset, global index),
+ * so the host gets the bits a device destination gets.
+ * A piece of a plain descriptor is the descriptor with elem_begin += l0 and elem_count = l1 - l0.  A piece
+ * of a windowed one (TDX_FLAG_WINDOW) keeps the window over its whole runs (elem_begin += (l0 / W) * P);
+ * a partial first or last run is a plain descriptor of that run's elements.
+ * Everything is validated before anything is enqueued: the descriptors as tdx_init_prepare checks them;
+ * a `dst` that CUDA reports as device (or managed) memory, a null, unaligned or too small staging buffer
+ * (smaller than one 16-byte vector plus the workspace of a one-descriptor pass) are TDX_E_BADARG.
+ * tdx_last_launch_count() then counts every pass's launches, tdx_last_host_copies() the copies.
+ */
+TDX_C_API int tdx_init_submit_host(const TdxInitDesc* descs, int n, void* staging, size_t staging_bytes,
+                                   void* stream);
+
+/* One piece of the cut of tdx_init_submit_host. */
+typedef struct TdxHostPiece {
+  int32_t desc;         /* index of its descriptor in the table */
+  int32_t pass;         /* the pass that writes it (0, 1, ...) */
+  uint64_t elem_first;  /* first local element of the descriptor it holds */
+  uint64_t elem_count;  /* its elements */
+  uint64_t staging_off; /* byte offset in the staging buffer (== dst + elem_first * itemsize, mod 16) */
+} TdxHostPiece;
+
+/*
+ * The cut tdx_init_submit_host makes of a table for a staging buffer of `staging_bytes`, without a device:
+ * the pieces in submission order (pass by pass).  Writes at most `max_pieces` of them into `pieces` (may
+ * be NULL) and the count and the number of passes into `*n_pieces` and `*n_passes`.  Validates the
+ * table as tdx_init_submit_host does, but for the memory type of `dst`.
+ */
+TDX_C_API int tdx_init_host_cut(const TdxInitDesc* descs, int n, size_t staging_bytes, TdxHostPiece* pieces,
+                                int max_pieces, int* n_pieces, int* n_passes);
+
+/*
+ * The descriptors (one to three) that write `piece` (of the descriptor `d`) into a staging buffer whose
+ * first byte is at `staging`, in local order; returns their number (negative: an error code).
+ */
+TDX_C_API int tdx_init_host_piece_descs(const TdxInitDesc* d, const TdxHostPiece* piece, void* staging,
+                                        TdxInitDesc out[3]);
+
+/* Device-to-host copies the last tdx_init_submit_host on this thread enqueued (one per piece). */
+TDX_C_API int tdx_last_host_copies(void);
+
 /* Number of kernel launches the last tdx_plan_launch/tdx_init_launch on this
  * thread issued (one per non-empty kernel family). */
 TDX_C_API int tdx_last_launch_count(void);

@@ -37,6 +37,7 @@ TDX_MAX_EPI = 4
 TDX_EPI_NOROUND = 0x100
 TDX_FLAG_SRC_NOROUND = 0x1
 TDX_FLAG_WINDOW = 0x2
+TDX_E_BADARG, TDX_E_WORKSPACE, TDX_E_NODEVICE = -1, -2, -3
 
 EXPORTED_SYMBOLS = (
     "tdx_init_workspace_bytes",
@@ -45,6 +46,10 @@ EXPORTED_SYMBOLS = (
     "tdx_init_submit",
     "tdx_plan_upload",
     "tdx_plan_launch",
+    "tdx_init_submit_host",
+    "tdx_init_host_cut",
+    "tdx_init_host_piece_descs",
+    "tdx_last_host_copies",
     "tdx_last_launch_count",
     "tdx_last_upload_bytes",
     "tdx_elems_per_block",
@@ -80,6 +85,16 @@ class TdxPlan(ctypes.Structure):
     _fields_ = [("opaque", ctypes.c_uint64 * 512)]
 
 
+class TdxHostPiece(ctypes.Structure):
+    _fields_ = [
+        ("desc", ctypes.c_int32),
+        ("pass_", ctypes.c_int32),
+        ("elem_first", ctypes.c_uint64),
+        ("elem_count", ctypes.c_uint64),
+        ("staging_off", ctypes.c_uint64),
+    ]
+
+
 assert ctypes.sizeof(TdxInitDesc) == 128, ctypes.sizeof(TdxInitDesc)
 
 _lib: Optional[ctypes.CDLL] = None
@@ -112,6 +127,17 @@ def load() -> ctypes.CDLL:
         ctypes.POINTER(TdxPlan)]
     lib.tdx_plan_launch.restype = ctypes.c_int
     lib.tdx_plan_launch.argtypes = [ctypes.POINTER(TdxPlan), ctypes.c_void_p, ctypes.c_void_p]
+    lib.tdx_init_submit_host.restype = ctypes.c_int
+    lib.tdx_init_submit_host.argtypes = [
+        ctypes.POINTER(TdxInitDesc), ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
+    lib.tdx_init_host_cut.restype = ctypes.c_int
+    lib.tdx_init_host_cut.argtypes = [
+        ctypes.POINTER(TdxInitDesc), ctypes.c_int, ctypes.c_size_t, ctypes.POINTER(TdxHostPiece), ctypes.c_int,
+        ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int)]
+    lib.tdx_init_host_piece_descs.restype = ctypes.c_int
+    lib.tdx_init_host_piece_descs.argtypes = [
+        ctypes.POINTER(TdxInitDesc), ctypes.POINTER(TdxHostPiece), ctypes.c_void_p, ctypes.POINTER(TdxInitDesc)]
+    lib.tdx_last_host_copies.restype = ctypes.c_int
     lib.tdx_last_launch_count.restype = ctypes.c_int
     lib.tdx_last_upload_bytes.restype = ctypes.c_size_t
     lib.tdx_elems_per_block.restype = ctypes.c_int
@@ -200,3 +226,34 @@ def submit(workspace_ptr: int, workspace_bytes: int, stream: int = 0) -> int:
     lib = load()
     check(lib.tdx_init_submit(workspace_ptr, workspace_bytes, stream))
     return lib.tdx_last_launch_count()
+
+
+def submit_host(descs: Sequence[TdxInitDesc], staging_ptr: int, staging_bytes: int, stream: int = 0) -> int:
+    """tdx_init_submit_host: runs a table of host destinations in passes through the device staging
+    buffer; returns the number of kernel launches over every pass."""
+    lib = load()
+    arr = (TdxInitDesc * len(descs))(*descs)
+    check(lib.tdx_init_submit_host(arr, len(descs), staging_ptr, staging_bytes, stream))
+    return lib.tdx_last_launch_count()
+
+
+def host_cut(descs: Sequence[TdxInitDesc], staging_bytes: int):
+    """tdx_init_host_cut, without a device: ``(pieces, passes)`` of the cut tdx_init_submit_host makes of
+    the table for a staging buffer of `staging_bytes` (``TdxHostPiece``s, pass by pass)."""
+    lib = load()
+    arr = (TdxInitDesc * len(descs))(*descs)
+    n, passes = ctypes.c_int(0), ctypes.c_int(0)
+    check(lib.tdx_init_host_cut(arr, len(descs), staging_bytes, None, 0, ctypes.byref(n), ctypes.byref(passes)))
+    pieces = (TdxHostPiece * n.value)()
+    check(lib.tdx_init_host_cut(arr, len(descs), staging_bytes, pieces, n.value, ctypes.byref(n), ctypes.byref(passes)))
+    return list(pieces), passes.value
+
+
+def piece_descs(desc: TdxInitDesc, piece: TdxHostPiece, staging_ptr: int = 0) -> list:
+    """tdx_init_host_piece_descs: the descriptors that write `piece` of `desc` into a staging buffer at
+    `staging_ptr`, in local order."""
+    out = (TdxInitDesc * 3)()
+    k = load().tdx_init_host_piece_descs(ctypes.byref(desc), ctypes.byref(piece), staging_ptr, out)
+    if k < 0:
+        check(k)
+    return list(out[:k])

@@ -646,11 +646,253 @@ int launch_groups(const PlanHeader& hdr, void* image, cudaStream_t stream, int& 
   return 0;
 }
 
+// ---- host destinations: the cut into staged passes (tdx_init_submit_host) ----------------------------
+
+thread_local int g_last_host_copies = 0;
+
+bool windowed(const TdxInitDesc& d) { return d.reserved & TDX_FLAG_WINDOW; }
+uint64_t window_width(const TdxInitDesc& d) { return is_aten(d) ? d.fill_bits[0] & 0xffffffffull : d.fill_bits[0]; }
+uint64_t window_pitch(const TdxInitDesc& d) { return is_aten(d) ? d.fill_bits[0] >> 32 : d.fill_bits[1]; }
+
+// The descriptor of global elements [begin, begin + count) of `d`'s tensor as one plain range.
+TdxInitDesc plain_part(const TdxInitDesc& d, uint64_t begin, uint64_t count, void* dst) {
+  TdxInitDesc p = d;
+  p.dst = dst;
+  p.elem_begin = begin;
+  p.elem_count = count;
+  if (windowed(d)) {
+    p.reserved &= ~TDX_FLAG_WINDOW;
+    p.fill_bits[0] = 0;  // (ATen's stream keeps its grid stride in fill_bits[1])
+    if (!is_aten(d)) p.fill_bits[1] = 0;
+  }
+  return p;
+}
+
+// The descriptors that write local elements [first, first + count) of `d` at `dst`: one for a plain
+// descriptor; for a window a partial first run, the whole runs and a partial last run, as the planner
+// emits a window (planner_engine.cc emit_window).
+int piece_descs(const TdxInitDesc& d, uint64_t first, uint64_t count, unsigned char* dst, TdxInitDesc out[3]) {
+  const uint64_t isz = itemsize_of(d.dtype);
+  if (!windowed(d)) {
+    out[0] = plain_part(d, d.elem_begin + first, count, dst);
+    return 1;
+  }
+  const uint64_t W = window_width(d), P = window_pitch(d);
+  int k = 0;
+  uint64_t a = first;
+  const uint64_t b = first + count;
+  auto global = [&](uint64_t l) { return d.elem_begin + (l / W) * P + l % W; };
+  if (a % W) {
+    const uint64_t c = std::min(W - a % W, b - a);
+    out[k++] = plain_part(d, global(a), c, dst + (a - first) * isz);
+    a += c;
+  }
+  const uint64_t runs = (b - a) / W;
+  if (runs > 1) {
+    out[k] = d;
+    out[k].dst = dst + (a - first) * isz;
+    out[k].elem_begin = global(a);
+    out[k++].elem_count = runs * W;
+    a += runs * W;
+  } else if (runs == 1) {
+    out[k++] = plain_part(d, global(a), W, dst + (a - first) * isz);
+    a += W;
+  }
+  if (a < b) out[k++] = plain_part(d, global(a), b - a, dst + (a - first) * isz);
+  return k;
+}
+
+// The table family that would take a plain range of `d` if it were large enough (-1: none): such a piece
+// needs room for the table kernel's work list in its pass's workspace.
+int table_family_of(const TdxInitDesc& d) {
+  if (d.algo & TDX_ALGO_NOLUT) return -1;
+  const TdxInitDesc p = plain_part(d, d.elem_begin, kLutMinElems, d.dst);
+  const int f = family_of(p);
+  return f >= 0 && families()[f].lut ? f : -1;
+}
+
+// Bytes of workspace build_plan can use for a pass of `n` descriptors of which those of `tables`
+// distinct table families may take the table kernel: the same terms as plan_bytes, counted for this
+// pass (groups <= descriptors) instead of for the largest table.
+size_t pass_workspace_bytes(size_t n, size_t tables) {
+  const size_t groups = std::min(n, families().size());
+  const size_t images = (groups + kMaxGroups - 1) / kMaxGroups;
+  return images * (sizeof(PlanHeader) + kImageAlign) + groups * (sizeof(unsigned long long) + 15 + 127) +
+         n * (sizeof(unsigned long long) + sizeof(TdxInitDesc) + sizeof(uint4)) +
+         tables * ((kMaxListChunks + kMaxListTail) * sizeof(uint4) + 15 + (kMaxListCtas + 1) * sizeof(uint32_t));
+}
+
+// The cut of a table for a staging buffer of `staging_bytes` (see tdx_init_submit_host).  A pass's
+// plan workspace sits at the head of the buffer; its pieces are placed from the end down, each at the
+// highest offset that keeps its destination's address mod 16, until the next one would reach into the
+// workspace the pass needs with it.
+int host_cut(const TdxInitDesc* descs, int n, size_t staging_bytes, std::vector<TdxHostPiece>& pieces,
+             int& passes) {
+  pieces.clear();
+  passes = 0;
+  // (one vector at any address mod 16 above the workspace of a one-descriptor pass)
+  if (staging_bytes < pass_workspace_bytes(1, 0) + 32)
+    return fail(TDX_E_BADARG, "staging buffer smaller than one vector plus a one-descriptor pass's workspace");
+  size_t top = staging_bytes, in_pass = 0;  // lowest staging byte used by the pass; its descriptors
+  std::vector<int> tables;                  // table families the pass has room for
+  bool open = false;
+  for (int i = 0; i < n; ++i) {
+    const TdxInitDesc& d = descs[i];
+    const uint64_t isz = itemsize_of(d.dtype);
+    const int table = table_family_of(d);
+    uint64_t l = 0;
+    while (l < d.elem_count) {
+      if (!open) {
+        top = staging_bytes;
+        in_pass = 0;
+        tables.clear();
+        open = true;
+        ++passes;
+      }
+      const uint64_t m = (reinterpret_cast<uintptr_t>(d.dst) + l * isz) % 16, rest = d.elem_count - l;
+      // elements that fit above a workspace of `ws` bytes, at an offset congruent to m
+      auto fit = [&](size_t ws) -> uint64_t {
+        const size_t base = ((ws + 15 - m) & ~static_cast<size_t>(15)) + m;
+        return base < top ? (top - base) / isz : 0;
+      };
+      const bool have_table = table >= 0 && std::find(tables.begin(), tables.end(), table) != tables.end();
+      // a piece of a window can be three descriptors; one run's part of it is one
+      uint64_t c = fit(pass_workspace_bytes(in_pass + (windowed(d) ? 3 : 1), tables.size()));
+      int nd = windowed(d) ? 3 : 1;
+      if (c == 0 && windowed(d)) {
+        c = std::min(fit(pass_workspace_bytes(in_pass + 1, tables.size())), window_width(d) - l % window_width(d));
+        nd = 1;
+      }
+      c = std::min(c, rest);
+      bool add_table = false;
+      if (table >= 0 && !have_table && c >= kLutMinElems) {  // large enough for the table kernel
+        const uint64_t t = std::min<uint64_t>(fit(pass_workspace_bytes(in_pass + nd, tables.size() + 1)), rest);
+        if (t >= kLutMinElems) {
+          c = t;
+          add_table = true;
+        } else {
+          c = kLutMinElems - 1;
+        }
+      }
+      if (c == 0) {
+        if (in_pass == 0) return fail(TDX_E_BADARG, "internal: a pass has no room for one element");
+        open = false;  // the next pass takes it
+        continue;
+      }
+      if (add_table) tables.push_back(table);
+      const size_t off = ((top - c * isz - m) & ~static_cast<size_t>(15)) + m;
+      pieces.push_back(TdxHostPiece{i, passes - 1, l, c, off});
+      top = off;
+      in_pass += nd;
+      l += c;
+    }
+  }
+  return 0;
+}
+
 }  // namespace tdx
 
 extern "C" {
 
 TDX_C_API size_t tdx_init_workspace_bytes(int n) { return tdx::plan_bytes(n < 0 ? 0 : n); }
+
+TDX_C_API int tdx_init_host_cut(const TdxInitDesc* descs, int n, size_t staging_bytes, TdxHostPiece* pieces,
+                                int max_pieces, int* n_pieces, int* n_passes) {
+  if (n_pieces == nullptr || n_passes == nullptr) return tdx::fail(TDX_E_BADARG, "n_pieces / n_passes == NULL");
+  {
+    thread_local std::vector<unsigned char> img;
+    thread_local tdx::PlanSet plans;
+    size_t used = 0;
+    if (int rc = tdx::build_plan(descs, n, img, plans, used)) return rc;
+  }
+  std::vector<TdxHostPiece> cut;
+  int passes = 0;
+  if (int rc = tdx::host_cut(descs, n, staging_bytes, cut, passes)) return rc;
+  if (pieces)
+    memcpy(pieces, cut.data(), std::min<size_t>(cut.size(), max_pieces < 0 ? 0 : max_pieces) * sizeof(TdxHostPiece));
+  *n_pieces = static_cast<int>(cut.size());
+  *n_passes = passes;
+  return 0;
+}
+
+TDX_C_API int tdx_init_host_piece_descs(const TdxInitDesc* d, const TdxHostPiece* piece, void* staging,
+                                        TdxInitDesc out[3]) {
+  if (d == nullptr || piece == nullptr || out == nullptr) return tdx::fail(TDX_E_BADARG, "NULL argument");
+  if (tdx::itemsize_of(d->dtype) == 0) return tdx::fail(TDX_E_BADARG, "unknown dtype");
+  if (piece->elem_count == 0 || piece->elem_first + piece->elem_count > d->elem_count)
+    return tdx::fail(TDX_E_BADARG, "the piece is not inside its descriptor");
+  if (tdx::windowed(*d) && tdx::window_width(*d) == 0) return tdx::fail(TDX_E_BADARG, "TDX_FLAG_WINDOW: W == 0");
+  return tdx::piece_descs(*d, piece->elem_first, piece->elem_count,
+                          static_cast<unsigned char*>(staging) + piece->staging_off, out);
+}
+
+TDX_C_API int tdx_init_submit_host(const TdxInitDesc* descs, int n, void* staging, size_t staging_bytes,
+                                   void* stream) {
+  tdx::g_last_launches = 0;
+  tdx::g_last_host_copies = 0;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (staging == nullptr || reinterpret_cast<uintptr_t>(staging) % 16)
+    return tdx::fail(TDX_E_BADARG, "staging == NULL or not 16-byte aligned");
+  thread_local std::vector<unsigned char> img;
+  thread_local tdx::PlanSet plans;
+  size_t used = 0;
+  if (int rc = tdx::build_plan(descs, n, img, plans, used)) return rc;
+  {
+    cudaPointerAttributes attr;
+    if (cudaPointerGetAttributes(&attr, staging) != cudaSuccess || attr.type != cudaMemoryTypeDevice) {
+      cudaGetLastError();
+      return tdx::fail(TDX_E_BADARG, "staging is not device memory");
+    }
+    for (int i = 0; i < n; ++i) {
+      if (descs[i].elem_count == 0) continue;
+      if (cudaPointerGetAttributes(&attr, descs[i].dst) != cudaSuccess) {
+        cudaGetLastError();
+        return tdx::fail(TDX_E_BADARG, "cudaPointerGetAttributes(dst) failed");
+      }
+      if (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged)
+        return tdx::fail(TDX_E_BADARG, "tdx_init_submit_host: dst is device memory (tdx_init_launch takes it)");
+    }
+  }
+  std::vector<TdxHostPiece> cut;
+  int passes = 0;
+  if (int rc = tdx::host_cut(descs, n, staging_bytes, cut, passes)) return rc;
+  // every pass's table, laid out before anything is enqueued (its workspace must fit under its pieces)
+  std::vector<std::vector<TdxInitDesc>> tables(static_cast<size_t>(passes));
+  std::vector<size_t> floor(static_cast<size_t>(passes), staging_bytes);
+  auto* base = static_cast<unsigned char*>(staging);
+  for (const TdxHostPiece& p : cut) {
+    TdxInitDesc part[3];
+    const int k = tdx::piece_descs(descs[p.desc], p.elem_first, p.elem_count, base + p.staging_off, part);
+    tables[p.pass].insert(tables[p.pass].end(), part, part + k);
+    floor[p.pass] = std::min<size_t>(floor[p.pass], p.staging_off);
+  }
+  for (int p = 0; p < passes; ++p) {
+    if (int rc = tdx::build_plan(tables[p].data(), static_cast<int>(tables[p].size()), img, plans, used)) return rc;
+    if (used > floor[p]) return tdx::fail(TDX_E_WORKSPACE, "internal: a pass's workspace reaches into its pieces");
+  }
+  size_t next = 0;
+  int launches = 0;
+  for (int p = 0; p < passes; ++p) {
+    if (int rc = tdx::build_plan(tables[p].data(), static_cast<int>(tables[p].size()), img, plans, used)) return rc;
+    tdx::g_last_upload_bytes = used;
+    void* pinned = nullptr;
+    if (int rc = tdx::stage(img.data(), used, s, staging, &pinned)) return rc;
+    for (size_t q = 0; q < plans.hdrs.size(); ++q)
+      if (int rc = tdx::launch_groups(plans.hdrs[q], base + plans.base[q], s, launches)) return rc;
+    for (; next < cut.size() && cut[next].pass == p; ++next) {
+      const TdxHostPiece& c = cut[next];
+      const size_t isz = tdx::itemsize_of(descs[c.desc].dtype);
+      cudaError_t e = cudaMemcpyAsync(static_cast<unsigned char*>(descs[c.desc].dst) + c.elem_first * isz,
+                                      base + c.staging_off, c.elem_count * isz, cudaMemcpyDeviceToHost, s);
+      if (e != cudaSuccess) return tdx::cuda_fail(e, "cudaMemcpyAsync(device to host)");
+      ++tdx::g_last_host_copies;
+    }
+  }
+  tdx::g_last_launches = launches;
+  return 0;
+}
+
+TDX_C_API int tdx_last_host_copies(void) { return tdx::g_last_host_copies; }
 
 TDX_C_API int tdx_plan_upload(const TdxInitDesc* descs, int n, void* workspace,
                               size_t workspace_bytes, void* stream, TdxPlan* plan) {

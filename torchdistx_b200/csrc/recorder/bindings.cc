@@ -374,6 +374,8 @@ py::dict py_last_stats() {
   d["generic_ops"] = s.generic_ops;
   d["narrowed_tensors"] = s.narrowed_tensors;
   d["aten_stream_tensors"] = s.aten_stream_tensors;
+  d["host_bytes"] = s.host_bytes;
+  d["host_copies"] = s.host_copies;
   d["elided_rng_ops"] = s.elided_rng_ops;
   d["kernel_launches"] = s.kernel_launches;
   d["bytes_written"] = s.bytes_written;

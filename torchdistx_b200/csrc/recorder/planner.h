@@ -77,6 +77,8 @@ struct MaterializeStats {
   int64_t prebuilt_outputs = 0;  // outputs the calling thread had built before the helper planned them
   int64_t narrowed_tensors = 0;  // Shard(d >= 1) tensors built whole and narrowed (index, table, copy programs)
   int64_t aten_stream_tensors = 0;  // fused tensors with a draw in ATen's stream (RngStream::Aten)
+  int64_t host_bytes = 0;   // bytes built into host memory (a CPU `out`: tdx_init_submit_host)
+  int64_t host_copies = 0;  // ... and the device-to-host copies that moved them
 };
 
 // Materialises `fake` (a no-op returning `fake` itself for real tensors).

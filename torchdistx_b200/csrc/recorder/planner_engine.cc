@@ -55,11 +55,24 @@ struct Slab {
 };
 void slab_ref_delete(void* ctx) { delete static_cast<std::shared_ptr<Slab>*>(ctx); }
 
+// Bytes of one element of a descriptor's destination (include/tdx_init.h dtypes).
+size_t itemsize_of(uint8_t dtype) {
+  switch (dtype) {
+    case TDX_F32: case TDX_RAW32: return 4;
+    case TDX_BF16: case TDX_F16: case TDX_RAW16: return 2;
+    case TDX_RAW8: return 1;
+    default: return 8;  // TDX_I64, TDX_RAW64
+  }
+}
+
 std::atomic<uint64_t> g_epoch{1};  // process-wide: storages remember the epoch across sessions
 
 struct Batch {
   c10::Device device = c10::Device(c10::kCPU);
   std::vector<TdxInitDesc> descs;
+  // The descriptors' destinations are host memory (a CPU `out` of a flat shard: FSDP1's offload_params):
+  // flush() runs them through tdx_init_submit_host.  A batch never mixes the two: flush before switching.
+  bool host = false;
   // Outputs whose memory is assigned at the next submission: the tensor object exists as soon as
   // its program has been planned (the caller can give it its Python identity meanwhile), its
   // storage gets its address when the slab is allocated.
@@ -267,17 +280,30 @@ void Batch::flush() {
     gather_dev.copy_(host, /*non_blocking=*/true);
     gathers.clear();
   }
-  // prepare: the plan is laid out on the host and says how much workspace it needs (descriptor table
-  // + prefix sums + work lists: tens of KB, not the upper bound of tdx_init_workspace_bytes)
-  size_t ws_bytes = 0;
-  int rc = tdx_init_prepare(descs.data(), n, &ws_bytes);
-  TORCH_CHECK(rc == 0, "libtdx_init: plan failed (", rc, "): ", tdx_last_error());
-  // (straight from the caching allocator: freed at the end of this scope, reused in stream order)
-  at::Tensor ws = at::detail::empty_cuda({static_cast<int64_t>(std::max<size_t>(ws_bytes, 16))}, at::kByte,
-                                         device, std::nullopt);
   auto stream = c10::cuda::getCurrentCUDAStream(device.index());
-  rc = tdx_init_submit(ws.data_ptr(), ws_bytes, stream.stream());
-  TORCH_CHECK(rc == 0, "libtdx_init: launch failed (", rc, "): ", tdx_last_error());
+  if (host) {
+    // host destinations: built in passes through one staging buffer of at most the first submission's
+    // size (flush_threshold's start), and never more than the whole table needs
+    size_t need = tdx_init_workspace_bytes(3 * n);
+    for (const TdxInitDesc& d : descs) need += d.elem_count * itemsize_of(d.dtype) + 16;
+    const size_t staging_bytes = std::min<size_t>(need, size_t{256} << 20);
+    at::Tensor staging = at::detail::empty_cuda({static_cast<int64_t>(staging_bytes)}, at::kByte, device, std::nullopt);
+    const int rc = tdx_init_submit_host(descs.data(), n, staging.data_ptr(), staging_bytes, stream.stream());
+    TORCH_CHECK(rc == 0, "libtdx_init: host submission failed (", rc, "): ", tdx_last_error());
+    g_stats.host_copies += tdx_last_host_copies();
+    for (const TdxInitDesc& d : descs) g_stats.host_bytes += static_cast<int64_t>(d.elem_count * itemsize_of(d.dtype));
+  } else {
+    // prepare: the plan is laid out on the host and says how much workspace it needs (descriptor table
+    // + prefix sums + work lists: tens of KB, not the upper bound of tdx_init_workspace_bytes)
+    size_t ws_bytes = 0;
+    int rc = tdx_init_prepare(descs.data(), n, &ws_bytes);
+    TORCH_CHECK(rc == 0, "libtdx_init: plan failed (", rc, "): ", tdx_last_error());
+    // (straight from the caching allocator: freed at the end of this scope, reused in stream order)
+    at::Tensor ws = at::detail::empty_cuda({static_cast<int64_t>(std::max<size_t>(ws_bytes, 16))}, at::kByte,
+                                           device, std::nullopt);
+    rc = tdx_init_submit(ws.data_ptr(), ws_bytes, stream.stream());
+    TORCH_CHECK(rc == 0, "libtdx_init: launch failed (", rc, "): ", tdx_last_error());
+  }
   g_stats.kernel_launches += tdx_last_launch_count();
   g_stats.descriptors += n;
   g_stats.submissions++;
@@ -852,7 +878,14 @@ struct Engine {
     at::Tensor out;
     Batch::Pending pend;
     char* abs_base = nullptr;
-    if (out_opt && out_opt->defined()) {
+    const bool host_out = out_opt && out_opt->defined() && out_opt->device().is_cpu();
+    if (host_out) {  // FSDP1's flat_param._local_shard under offload_params: built on *dev, copied to the host
+      out = *out_opt;
+      TORCH_CHECK_VALUE(out.scalar_type() == dtype && out.dim() == 1 && out.is_contiguous() && out.numel() >= chunk,
+                        "flat shard: a CPU `out` must be a contiguous 1-D tensor of the parameters' dtype with at "
+                        "least ceil(total / world) elements");
+      abs_base = static_cast<char*>(out.data_ptr());
+    } else if (out_opt && out_opt->defined()) {
       out = *out_opt;
       TORCH_CHECK_VALUE(out.is_cuda() && out.device() == *dev && out.scalar_type() == dtype && out.dim() == 1 &&
                             out.is_contiguous() && out.numel() >= chunk,
@@ -920,9 +953,10 @@ struct Engine {
             break;
           }
     }
-    if (batch.device != *dev) {
+    if (batch.device != *dev || batch.host != host_out) {
       batch.flush();
       batch.device = *dev;
+      batch.host = host_out;
     }
     pend.first_desc = static_cast<uint32_t>(batch.descs.size());
     // Pass 2: this chunk's descriptors (nothing else touches the batch from here to the flush)
@@ -949,10 +983,15 @@ struct Engine {
     g_stats.bytes_written += bytes;
     g_stats.fused_tensors += static_cast<int64_t>(items.size() - deferred.size());
     batch.flush();
+    batch.host = false;
     if (!deferred.empty()) {
       NoInterception guard;
       for (const Deferred& d : deferred)
         out.narrow(0, d.dst_begin - lo, d.count).copy_(d.full.reshape({-1}).narrow(0, d.src_begin, d.count));
+    }
+    if (host_out) {  // (copies into pinned memory are asynchronous: the caller reads `out` on the host next)
+      const cudaError_t e = cudaStreamSynchronize(c10::cuda::getCurrentCUDAStream(dev->index()).stream());
+      TORCH_CHECK(e == cudaSuccess, "flat shard: ", cudaGetErrorString(e));
     }
     return out;
   }

@@ -295,6 +295,12 @@ def materialize_flat_shard(
     any time.  Returns ``(local_shard, offsets)``: ``offsets[i]`` is the start of ``params[i]`` in
     the flat parameter, ``offsets[-1]`` its unpadded total.
 
+    ``out`` may be a CPU tensor, pinned or pageable: FSDP1's ``_local_shard`` under
+    ``CPUOffload(offload_params=True)``.  The chunk is still built on the parameters' CUDA device and
+    copied to host memory in passes through a bounded staging buffer (``tdx_init_submit_host``), with
+    the bits a CUDA ``out`` gets; the call returns once ``out`` holds them.  ``last_materialize_stats()``
+    counts the bytes and copies as ``host_bytes`` and ``host_copies``.
+
     The parameters stay deferred; all ranks must hold the same generator state
     (:func:`torchdistx_b200.parallel.sync_rng`) and pass the same list.  ``rng``: see
     :func:`materialize_module`.

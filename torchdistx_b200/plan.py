@@ -63,6 +63,11 @@ FORMAT_ATEN = "torchdistx_b200.InitPlan/7"
 _FORMATS = (FORMAT_ATEN, FORMAT_BAND, FORMAT_GATHER, FORMAT_SINCOS, FORMAT_SSM, FORMAT, "torchdistx_b200.InitPlan/1")
 
 
+# Staging for host targets: the engine's first submission size (planner_engine.cc), and never more than
+# one pass of the table needs.
+HOST_STAGING_BYTES = 256 << 20
+
+
 def offset_increment(numel: int) -> int:
     """Generator offset one RNG pass over `numel` elements consumes (planner_engine.cc assign_rng)."""
     blocks = (numel + 3) // 4
@@ -584,7 +589,8 @@ class InitPlan:
                     generator: Optional[torch.Generator] = None,
                     into: Optional[Dict[str, torch.Tensor]] = None,
                     placements: Optional[Dict[str, Optional[int]]] = None,
-                    blocks: Optional[Dict[str, Steps]] = None) -> Dict[str, torch.Tensor]:
+                    blocks: Optional[Dict[str, Steps]] = None,
+                    staging_bytes: int = HOST_STAGING_BYTES) -> Dict[str, torch.Tensor]:
         """Builds every tensor of the plan on `device` through libtdx_init and returns
         ``{name: tensor}`` (parameters as ``torch.nn.Parameter``).  Consumes the CUDA generator
         exactly like ``materialize_module`` would.
@@ -594,6 +600,14 @@ class InitPlan:
         the FSDP hand-off of SURVEY 8f.1: after ``fully_shard(meta_model)`` / ``to_empty`` the
         local shards FSDP owns are initialised in place, no unsharded tensor, no copy
         (:func:`init_sharded_module`).
+
+        An `into` buffer may also be a contiguous CPU tensor, pinned or pageable: a CPU-offloaded shard
+        (FSDP2's ``CPUOffloadPolicy``, FSDP1's ``offload_params``).  Its descriptors are built on `device`
+        all the same and copied to host memory in passes through a staging buffer of at most
+        `staging_bytes` (``tdx_init_submit_host``), after the table of device targets; by-value entries
+        and entries built whole and narrowed are built on the device and copied into it.  The bits and
+        the generator offsets are those of CUDA targets.  The call returns once every host target holds
+        its values.
 
         `placements`: a tensor-parallel layout, as for :meth:`descriptors` (the tensors are this
         rank's local blocks; entries built whole and narrowed are narrowed here, on the device).
@@ -617,6 +631,8 @@ class InitPlan:
             aten = props.multi_processor_count, props.max_threads_per_multi_processor
         out: Dict[str, torch.Tensor] = {}
         descs = []
+        host_descs = []  # descriptors whose destination is a CPU `into` buffer
+        host_written = False
         staged: List[torch.Tensor] = []  # gather sources on the device: alive until the launch is queued
 
         def gather_src(g: dict) -> int:
@@ -637,6 +653,7 @@ class InitPlan:
                     t = value_tensor(e, steps=steps).to(device)
                     if target is not None:
                         target.copy_(t)
+                        host_written |= target.device.type == "cpu"
                         t = target
                     out[e.name] = t if target is not None else _wrap(t, e)
                     continue
@@ -644,7 +661,12 @@ class InitPlan:
                     narrow.append((e, block_ranges(list(e.sizes), steps)))
                     steps, target = [], None  # (the whole tensor is a temporary)
                 begin, count, sizes = shard_range(e, steps=steps)
-                if target is not None:
+                if target is not None and target.device.type == "cpu":
+                    if not (target.is_contiguous() and target.dtype == dtype and target.numel() >= count):
+                        raise ValueError(f"'{e.name}': a CPU `into` buffer must be a contiguous {dtype} tensor "
+                                         f"with at least {count} elements")
+                    t = target
+                elif target is not None:
                     if not (target.is_cuda and target.is_contiguous() and target.dtype == dtype
                             and target.numel() >= count):
                         raise ValueError(f"'{e.name}': `into` buffer must be a contiguous CUDA {dtype} tensor "
@@ -653,7 +675,8 @@ class InitPlan:
                 else:
                     t = torch.empty(sizes, dtype=dtype, device=device)
                 pass_offset, offset = assign_pass_offsets(e, assigned, offset, aten)
-                descs += entry_descriptors(e, t.data_ptr(), begin, count, seed, pass_offset, gather_src,
+                table = host_descs if t.device.type == "cpu" else descs
+                table += entry_descriptors(e, t.data_ptr(), begin, count, seed, pass_offset, gather_src,
                                            shard_window(e, steps=steps), aten)
                 out[e.name] = t if target is not None else _wrap(t, e)
             if descs:
@@ -661,13 +684,19 @@ class InitPlan:
                 if ws_bytes:
                     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
                     _cabi.submit(ws.data_ptr(), ws_bytes, torch.cuda.current_stream(device).cuda_stream)
+            if host_descs:
+                submit_host(host_descs, device, staging_bytes)
+                host_written = True
             for e, ranges in narrow:
                 t = _narrow(out[e.name].detach(), ranges).contiguous()
                 target = None if into is None else into.get(e.name)
                 if target is not None:
                     target.view(-1)[: t.numel()].copy_(t.view(-1))
+                    host_written |= target.device.type == "cpu"
                 out[e.name] = target if target is not None else _wrap(t, e)
             gen.set_offset(offset)
+            if host_written:  # (pinned copies are asynchronous: the host reads these tensors next)
+                torch.cuda.current_stream(device).synchronize()
         return out
 
     def apply(self, module: Module, **kw) -> None:
@@ -679,6 +708,25 @@ class InitPlan:
             mod = module.get_submodule(owner) if owner else module
             group = mod._parameters if key in mod._parameters else mod._buffers
             group[key] = t
+
+
+def host_staging_bytes(descs, staging_bytes: int = HOST_STAGING_BYTES) -> int:
+    """The staging buffer :func:`submit_host` allocates for `descs`: `staging_bytes`, or less when the
+    whole table (its bytes, each piece's alignment and the workspace of one pass) fits in less."""
+    item = {_cabi.TDX_F32: 4, _cabi.TDX_BF16: 2, _cabi.TDX_F16: 2, _cabi.TDX_I64: 8, _cabi.TDX_RAW8: 1,
+            _cabi.TDX_RAW16: 2, _cabi.TDX_RAW32: 4, _cabi.TDX_RAW64: 8}
+    data = sum(int(d.elem_count) * item[int(d.dtype)] + 16 for d in descs)
+    return min(int(staging_bytes), data + _cabi.load().tdx_init_workspace_bytes(3 * len(descs)))
+
+
+def submit_host(descs, device: torch.device, staging_bytes: int = HOST_STAGING_BYTES) -> int:
+    """Runs a table of host destinations through ``tdx_init_submit_host`` on `device`'s current stream,
+    with a staging buffer from the caching allocator; returns the kernel launches over every pass.  The
+    copies into pinned memory are asynchronous: synchronise the stream before reading the targets."""
+    n = host_staging_bytes(descs, staging_bytes)
+    stream = torch.cuda.current_stream(device)
+    staging = torch.empty(n, dtype=torch.uint8, device=device)  # (freed in stream order after the copies)
+    return _cabi.submit_host(descs, staging.data_ptr(), n, stream.cuda_stream)
 
 
 def _wrap(t: torch.Tensor, e: PlanEntry) -> torch.Tensor:
