@@ -5,17 +5,22 @@
  * product (torchdistx_b200) never does and has no CPU path for CUDA tensors.
  *
  * What is restated, and against what it is pinned:
- *   philox4x32_R     the Philox4x32 generator ATen/curand use on CUDA.  Published algorithm:
- *                    Salmon, Moraes, Dror, Shaw, SC'11 (Random123 1.x).  Dependency of the
- *                    reference path: PyTorch (un-vendored; pinned here: torch 2.11.0+cu128,
+ *   philox4x32_R     the Philox4x32 generator ATen/curand use on CUDA (tdx_philox.c).  Published
+ *                    algorithm: Salmon, Moraes, Dror, Shaw, SC'11 (Random123 1.x).  Dependency of
+ *                    the reference path: PyTorch (un-vendored; pinned here: torch 2.11.0+cu128,
  *                    $TORCH/include/ATen/core/PhiloxRNGEngine.h:60-220).  Pinned by
  *                    tests/golden/philox_kat.json = Random123 known-answer vectors + outputs of
  *                    at::Philox4_32 itself (tests/golden/make_philox_kat.py).
  *   transforms       element g of a tensor := f(seed, offset, g) exactly as
- *                    torchdistx_b200/csrc/kernels/tdx_device.cuh and tdx_init_kernels.cu compute
- *                    it, with libm in place of the MUFU approximations (lg2/sqrt/sin/cos), so RNG
- *                    floats agree to the tolerance stated in tests/test_kernels_gpu.py and everything else
+ *                    torchdistx_b200/csrc/kernels compute it, for every descriptor of
+ *                    include/tdx_init.h (tdx_oracle_generate): constants, the fused uniform and
+ *                    normal generators, windows, index programs, sinusoid tables, copies of host
+ *                    arrays, band masks and every epilogue step.  libm stands in for the MUFU
+ *                    approximations (lg2/sqrt/sin/cos) and for libdevice's exp/log/expm1/erfinv, so
+ *                    those floats agree to the tolerances the tests state, and everything else
  *                    (constants, uniform, rounding, epilogue arithmetic, sharding) bit for bit.
+ *   ATen's stream    TDX_ALGO_ATEN(_WIDE) draws: the unit uniform / normal of each element
+ *                    (tdx_oracle_aten_units, on tdx_philox.c); tdx_oracle_generate rejects them.
  *   semantics        what uniform_/normal_/fill_ MEAN follows ATen, the arithmetic owner of the
  *                    reference's replay (reference src/cc/torchdistx/deferred_init.cc:218-220):
  *                    bounds cast to the tensor dtype, value = u*(to-from)+from, half-open range
@@ -30,24 +35,7 @@
 #include <string.h>
 
 #include "tdx_init.h"
-
-#define PHILOX_M0 0xD2511F53u
-#define PHILOX_M1 0xCD9E8D57u
-#define PHILOX_W0 0x9E3779B9u
-#define PHILOX_W1 0xBB67AE85u
-
-/* out[4] = Philox4x32-`rounds`(counter ctr[4], key[2]) */
-void tdx_oracle_philox4x32(const uint32_t ctr[4], const uint32_t key[2], int rounds, uint32_t out[4]) {
-  uint32_t c0 = ctr[0], c1 = ctr[1], c2 = ctr[2], c3 = ctr[3], k0 = key[0], k1 = key[1];
-  for (int r = 0; r < rounds; ++r) {
-    const uint64_t p0 = (uint64_t)c0 * PHILOX_M0, p1 = (uint64_t)c2 * PHILOX_M1;
-    const uint32_t n0 = (uint32_t)(p1 >> 32) ^ c1 ^ k0, n1 = (uint32_t)p1;
-    const uint32_t n2 = (uint32_t)(p0 >> 32) ^ c3 ^ k1, n3 = (uint32_t)p0;
-    c0 = n0; c1 = n1; c2 = n2; c3 = n3;
-    k0 += PHILOX_W0; k1 += PHILOX_W1;
-  }
-  out[0] = c0; out[1] = c1; out[2] = c2; out[3] = c3;
-}
+#include "tdx_philox.c"
 
 /* the engine's counter layout (include/tdx_init.h "Random stream specification") */
 static void block_of(const TdxInitDesc* d, uint64_t blk, uint32_t wflag, uint32_t out[4]) {
@@ -141,20 +129,41 @@ static double ndtri(double p) {
   return q < 0 ? -num / den : num / den;
 }
 
-static float apply_epi(const TdxInitDesc* d, float v) {
-  if (!(d->reserved & TDX_FLAG_SRC_NOROUND)) v = round_through(v, d->dtype);
+/* kernel: apply_epi<Out> (and, for index programs, sinusoid columns and fp32 copies, apply_epi<float>:
+ * `dtype` is the type each step rounds to).  expf / logf / expm1f and the double ndtri for erfinv are
+ * C libm's, each within a few ulp of the CUDA libdevice functions the kernels call, not their bits. */
+static float apply_epi(const TdxInitDesc* d, float v, int dtype) {
+  if (!(d->reserved & TDX_FLAG_SRC_NOROUND)) v = round_through(v, dtype);
   for (int i = 0; i < d->n_epi && i < TDX_MAX_EPI; ++i) {
     const uint32_t op = d->epi[i].op;
+    const int rnd = !(op & TDX_EPI_NOROUND);
+    const float a = d->epi[i].a, b = d->epi[i].b;
     switch (op & 0xffu) {
-      case TDX_EPI_MUL: v = v * d->epi[i].a; break;
-      case TDX_EPI_ADD: v = v + d->epi[i].a; break;
+      case TDX_EPI_MUL: v = v * a; break;
+      case TDX_EPI_ADD: v = v + a; break;
       case TDX_EPI_ERFINV: v = (float)(ndtri(((double)v + 1.0) * 0.5) * 0.70710678118654752440); break;
-      case TDX_EPI_CLAMP: v = isnan(v) ? v : fminf(fmaxf(v, d->epi[i].a), d->epi[i].b); break; /* clamp_ keeps a NaN */
-      case TDX_EPI_RPOW: v = powf(d->epi[i].a, v); break; /* libm vs CUDA powf: both ~1 ulp, not each other's bits */
+      case TDX_EPI_CLAMP: v = isnan(v) ? v : fminf(fmaxf(v, a), b); break; /* clamp_ keeps a NaN */
+      case TDX_EPI_RPOW: v = powf(a, v); break; /* libm vs CUDA powf: both ~1 ulp, not each other's bits */
       case TDX_EPI_RECIP: v = 1.0f / v; break;
+      case TDX_EPI_EXP: v = expf(v); break;
+      case TDX_EPI_LOG: v = logf(v); break;
+      case TDX_EPI_EXPM1: v = expm1f(v); break;
+      case TDX_EPI_INV_SOFTPLUS: { /* v + log(-expm1(-v)), rounded after each ATen op */
+        float t = expm1f(-v);
+        if (rnd) t = round_through(t, dtype);
+        t = logf(-t);
+        if (rnd) t = round_through(t, dtype);
+        v = v + t;
+        break;
+      }
+      case TDX_EPI_MULADD:
+        v = v * a;
+        if (rnd) v = round_through(v, dtype);
+        v = v + b;
+        break;
       default: break;
     }
-    if (!(op & TDX_EPI_NOROUND)) v = round_through(v, d->dtype);
+    if (rnd) v = round_through(v, dtype);
   }
   return v;
 }
@@ -184,7 +193,7 @@ static int resolve_algo(const TdxInitDesc* d) {
   return 0;
 }
 
-/* Value (fp32, before the rounding of the store) of GLOBAL element g of the descriptor's tensor. */
+/* The generated value (fp32, before any epilogue step) of GLOBAL element g of a random descriptor. */
 static float element(const TdxInitDesc* d, uint64_t g) {
   const int algo = resolve_algo(d);
   uint32_t w[4];
@@ -232,53 +241,175 @@ static float element(const TdxInitDesc* d, uint64_t g) {
       }
     }
   }
-  return d->n_epi ? apply_epi(d, v) : v;
+  return v;
+}
+
+static int itemsize(int dtype) {
+  switch (dtype) {
+    case TDX_RAW8: return 1;
+    case TDX_RAW16: case TDX_BF16: case TDX_F16: return 2;
+    case TDX_RAW32: case TDX_F32: return 4;
+    case TDX_RAW64: case TDX_I64: return 8;
+    default: return 0;
+  }
+}
+
+static int is_float(int dtype) { return dtype == TDX_F32 || dtype == TDX_BF16 || dtype == TDX_F16; }
+
+/* the store of a float output: one rounding */
+static void store_float(const TdxInitDesc* d, void* out, uint64_t i, float v) {
+  if (d->dtype == TDX_F32) ((float*)out)[i] = v;
+  else if (d->dtype == TDX_BF16) ((uint16_t*)out)[i] = f32_to_bf16(v);
+  else ((uint16_t*)out)[i] = f32_to_f16(v);
+}
+
+/* kernel: tdx_init_sincos.cu sincos_value.  sinf / cosf are C libm's, each within an ulp or two of the
+ * CUDA libdevice functions the kernel calls, not their bits. */
+static float sincos_element(const TdxInitDesc* d, uint64_t g) {
+  const uint64_t half = d->fill_bits[0], width = 2 * half;
+  const uint64_t r = g / width, c = g % width;
+  const int second = c >= half;
+  const uint64_t k = second ? c - half : c;
+  float f = (float)((int64_t)d->p0 + (int64_t)k * (int64_t)d->p1);
+  if (d->n_epi) f = apply_epi(d, f, TDX_F32); /* the column program runs in fp32 */
+  const float x = (float)r * f;
+  const int cos_first = (d->fill_bits[1] & TDX_SINCOS_COS_FIRST) != 0;
+  return second != cos_first ? cosf(x) : sinf(x);
 }
 
 /*
  * Fills `out` (host memory, elem_count elements of the descriptor's dtype) with what the GPU
- * kernels write for this descriptor.  Returns 0, or -1 for an unsupported descriptor.
+ * kernels write for this descriptor.  Returns 0, or -1 for a descriptor outside the restatement:
+ * ATen's stream included (tdx_oracle_aten_units restates its draws).
  */
 int tdx_oracle_generate(const TdxInitDesc* d, void* out) {
   if (d->algo & ~(0x0f | TDX_ALGO_NOLUT)) return -1; /* the library rejects unknown flags too */
-  if (d->src == TDX_SRC_CONST) {
-    const int isz = (d->dtype == TDX_F32 || d->dtype == TDX_RAW32) ? 4 : d->dtype == TDX_RAW64 ? 8
-                    : d->dtype == TDX_RAW8 ? 1 : 2;
-    unsigned char pat[16];
-    memcpy(pat, d->fill_bits, 16);
-    for (uint64_t i = 0; i < d->elem_count; ++i) memcpy((unsigned char*)out + i * isz, pat, isz);
-    return 0;
-  }
-  if (d->src == TDX_SRC_IOTA) { /* element g = p0 + g * p1 (integers), then the fp32 epilogue */
-    const int64_t start = (int64_t)d->p0, step = (int64_t)d->p1;
-    if (!(d->dtype == TDX_F32 || d->dtype == TDX_BF16 || d->dtype == TDX_F16 || (d->dtype == TDX_I64 && d->n_epi == 0)))
-      return -1;
-    for (uint64_t i = 0; i < d->elem_count; ++i) {
-      const int64_t val = start + (int64_t)(d->elem_begin + i) * step;
-      if (d->dtype == TDX_I64) { ((int64_t*)out)[i] = val; continue; }
-      float v = (float)val;
-      if (d->n_epi) { /* index programs run in fp32 whatever the output type (kernel: apply_epi<float>) */
-        TdxInitDesc f = *d;
-        f.dtype = TDX_F32;
-        v = apply_epi(&f, v);
-      }
-      if (d->dtype == TDX_F32) ((float*)out)[i] = v;
-      else if (d->dtype == TDX_BF16) ((uint16_t*)out)[i] = f32_to_bf16(v); /* one rounding, at the store */
-      else ((uint16_t*)out)[i] = f32_to_f16(v);
+  if (d->reserved & TDX_FLAG_WINDOW) {
+    /* the plain descriptors of its runs: run o is global elements [elem_begin + o * P, + W), written
+     * at local o * W */
+    const uint64_t W = d->fill_bits[0], P = d->fill_bits[1];
+    const int isz = itemsize(d->dtype);
+    if ((d->src != TDX_SRC_UNIFORM && d->src != TDX_SRC_NORMAL) || W == 0 || P < W) return -1;
+    for (uint64_t l = 0; l < d->elem_count; l += W) {
+      TdxInitDesc run = *d;
+      run.reserved &= ~TDX_FLAG_WINDOW;
+      run.fill_bits[0] = run.fill_bits[1] = 0;
+      run.elem_begin = d->elem_begin + (l / W) * P;
+      run.elem_count = d->elem_count - l < W ? d->elem_count - l : W;
+      if (tdx_oracle_generate(&run, (unsigned char*)out + l * isz)) return -1;
     }
     return 0;
   }
-  if (d->dtype != TDX_F32 && d->dtype != TDX_BF16 && d->dtype != TDX_F16) return -1;
-  {
-    const int algo = resolve_algo(d);
-    if (d->src == TDX_SRC_NORMAL && algo != TDX_ALGO_BM32 && !(algo == TDX_ALGO_ICDF16 && d->dtype != TDX_F32))
+  switch (d->src) {
+    case TDX_SRC_CONST: {
+      const int isz = itemsize(d->dtype);
+      unsigned char pat[16];
+      if (!isz) return -1;
+      memcpy(pat, d->fill_bits, 16);
+      for (uint64_t i = 0; i < d->elem_count; ++i) memcpy((unsigned char*)out + i * isz, pat, isz);
+      return 0;
+    }
+    case TDX_SRC_IOTA: { /* element g = p0 + g * p1 (integers), then the fp32 epilogue */
+      /* broadcast (fill_bits = {P, R}, P > 0): global element g indexes (g / R) % P */
+      const int64_t start = (int64_t)d->p0, step = (int64_t)d->p1;
+      const uint64_t period = d->fill_bits[0], repeat = d->fill_bits[1] ? d->fill_bits[1] : 1;
+      if (!(is_float(d->dtype) || (d->dtype == TDX_I64 && d->n_epi == 0))) return -1;
+      for (uint64_t i = 0; i < d->elem_count; ++i) {
+        uint64_t g = d->elem_begin + i;
+        if (period) g = (g / repeat) % period;
+        const int64_t val = start + (int64_t)g * step;
+        if (d->dtype == TDX_I64) { ((int64_t*)out)[i] = val; continue; }
+        float v = (float)val;
+        if (d->n_epi) v = apply_epi(d, v, TDX_F32); /* index programs run in fp32 whatever the output type */
+        store_float(d, out, i, v);
+      }
+      return 0;
+    }
+    case TDX_SRC_SINCOS:
+      if (!is_float(d->dtype)) return -1;
+      if (d->fill_bits[0] == 0 || (d->fill_bits[1] & ~(uint64_t)TDX_SINCOS_COS_FIRST)) return -1;
+      if (d->elem_count && (d->elem_begin + d->elem_count - 1) / (2 * d->fill_bits[0]) >= (1ull << 24)) return -1;
+      for (uint64_t i = 0; i < d->elem_count; ++i) store_float(d, out, i, sincos_element(d, d->elem_begin + i));
+      return 0;
+    case TDX_SRC_GATHER: { /* kernel: tdx_init_gather.cu gather_tiles; the source is a host address here */
+      const void* src = (const void*)(uintptr_t)d->fill_bits[0];
+      const uint64_t period = d->fill_bits[1] & 0xffffffffull, rep = d->fill_bits[1] >> 32;
+      if (!(is_float(d->dtype) || (d->dtype == TDX_I64 && d->n_epi == 0))) return -1;
+      if (src == NULL || d->algo || d->reserved || (period == 0 && rep != 0)) return -1;
+      for (uint64_t j = 0; j < d->elem_count; ++j) {
+        const uint64_t g = d->elem_begin + j;
+        const uint64_t i = period ? (g / (rep ? rep : 1)) % period : g;
+        if (d->dtype == TDX_I64) {
+          ((uint64_t*)out)[j] = ((const uint64_t*)src)[i];
+        } else if (d->dtype == TDX_F32) {
+          float v = ((const float*)src)[i];
+          if (d->n_epi) v = apply_epi(d, v, TDX_F32);
+          memcpy((uint32_t*)out + j, &v, 4); /* (the bits as they are without an epilogue) */
+        } else {
+          const uint16_t w = ((const uint16_t*)src)[i];
+          if (!d->n_epi) {
+            ((uint16_t*)out)[j] = w;
+            continue;
+          }
+          const float v = d->dtype == TDX_BF16 ? bf16_to_f32(w) : f16_to_f32(w);
+          store_float(d, out, j, apply_epi(d, v, d->dtype));
+        }
+      }
+      return 0;
+    }
+    case TDX_SRC_BAND: { /* kernel: tdx_init_band.cu band_tiles, element by element with its own division */
+      const int isz = itemsize(d->dtype);
+      const uint64_t C = d->fill_bits[0] & 0xffffffffull, R = d->fill_bits[0] >> 32;
+      const int64_t lo = (int32_t)(uint32_t)d->fill_bits[1], hi = (int32_t)(uint32_t)(d->fill_bits[1] >> 32);
+      if (!isz || C == 0 || R == 0 || C >= (1ull << 31) || R >= (1ull << 31) || lo > hi || d->n_epi || d->algo ||
+          d->reserved)
+        return -1;
+      for (uint64_t j = 0; j < d->elem_count; ++j) {
+        const uint64_t g = d->elem_begin + j;
+        const int64_t c = (int64_t)(g % C), r = (int64_t)((g / C) % R);
+        const uint64_t v = (lo <= c - r && c - r <= hi) ? d->philox_seed : d->philox_offset;
+        memcpy((unsigned char*)out + j * isz, &v, (size_t)isz); /* (the low bytes: little-endian) */
+      }
+      return 0;
+    }
+    case TDX_SRC_UNIFORM:
+    case TDX_SRC_NORMAL: {
+      const int algo = resolve_algo(d);
+      if (!is_float(d->dtype)) return -1;
+      if ((d->algo & 0x0f) == TDX_ALGO_ATEN || (d->algo & 0x0f) == TDX_ALGO_ATEN_WIDE) return -1;
+      if (d->src == TDX_SRC_NORMAL && algo != TDX_ALGO_BM32 && !(algo == TDX_ALGO_ICDF16 && d->dtype != TDX_F32))
+        return -1;
+      for (uint64_t i = 0; i < d->elem_count; ++i) {
+        float v = element(d, d->elem_begin + i);
+        if (d->n_epi) v = apply_epi(d, v, d->dtype);
+        store_float(d, out, i, v);
+      }
+      return 0;
+    }
+    default:
       return -1;
   }
-  for (uint64_t i = 0; i < d->elem_count; ++i) {
-    const float v = element(d, d->elem_begin + i);
-    if (d->dtype == TDX_F32) ((float*)out)[i] = v;
-    else if (d->dtype == TDX_BF16) ((uint16_t*)out)[i] = f32_to_bf16(v);
-    else ((uint16_t*)out)[i] = f32_to_f16(v);
+}
+
+/*
+ * ATen's stream (TDX_ALGO_ATEN, TDX_ALGO_ATEN_WIDE): out[l] = the unit draw -- aten_uniform01 or
+ * aten_normal01, before ATen's transform and the epilogue -- of local element l's global index, under
+ * the descriptor's window (fill_bits[0] = W | P << 32) if it has one; fill_bits[1] = S.  Returns 0, or
+ * -1 for another descriptor, S == 0, a bad window or a last global element >= 2^31.
+ */
+int tdx_oracle_aten_units(const TdxInitDesc* d, float* out) {
+  const int window = (d->reserved & TDX_FLAG_WINDOW) != 0;
+  const uint64_t W = window ? (d->fill_bits[0] & 0xffffffffull) : 1, P = window ? d->fill_bits[0] >> 32 : 1;
+  const uint32_t S = (uint32_t)d->fill_bits[1];
+  if ((d->src != TDX_SRC_UNIFORM && d->src != TDX_SRC_NORMAL) ||
+      (d->algo != TDX_ALGO_ATEN && d->algo != TDX_ALGO_ATEN_WIDE) || S == 0 || W == 0 || P < W)
+    return -1;
+  if (d->elem_count && d->elem_begin + ((d->elem_count - 1) / W) * P + (d->elem_count - 1) % W >= (1ull << 31))
+    return -1;
+  for (uint64_t l = 0; l < d->elem_count; ++l) {
+    const uint32_t g = (uint32_t)(d->elem_begin + (l / W) * P + l % W);
+    out[l] = d->src == TDX_SRC_NORMAL ? aten_normal01(d->philox_seed, d->philox_offset, S, g)
+                                      : aten_uniform01(d->philox_seed, d->philox_offset, S, g);
   }
   return 0;
 }

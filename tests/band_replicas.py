@@ -1,17 +1,9 @@
 """Replicas of the causal-mask builders of transformers 5.5 (GPT-BigCode, GPT-Neo, ImageGPT / Bark /
 CLVP, OpenAI GPT) and of the additive `full(-inf).triu(1)` mask, each as its module records it (the
-constructor's buffer and `_init_weights`' `copy_` over it), plus the CPU restatement of the band
-kernel (tests/band_oracle.c)."""
-import ctypes
-import os
-import subprocess
-import tempfile
-
+constructor's buffer and `_init_weights`' `copy_` over it)."""
 import numpy as np
 import torch
 from torch import nn
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def causal_bool(n: int) -> torch.Tensor:
@@ -73,38 +65,6 @@ class NeoStack(nn.Module):
     def __init__(self, layers=24, n=2048, window=256):
         super().__init__()
         self.h = nn.ModuleList(NeoAttentionMask(n, window if i % 2 else 0) for i in range(layers))
-
-
-_lib = None
-
-
-def oracle():
-    """tests/band_oracle.c, built once per process into a temporary directory."""
-    global _lib
-    if _lib is None:
-        so = os.path.join(tempfile.mkdtemp(prefix="tdx_band_oracle_"), "libband_oracle.so")
-        subprocess.run(["gcc", "-O2", "-fPIC", "-std=c11", "-ffp-contract=off", "-fno-fast-math", "-shared",
-                        "-I" + os.path.join(ROOT, "include"), "-I" + os.path.join(ROOT, "oracle"),
-                        "-I" + os.path.join(ROOT, "tests"), "-o", so,
-                        os.path.join(ROOT, "tests", "band_oracle.c"), "-lm"], check=True)
-        _lib = ctypes.CDLL(so)
-        _lib.tdx_oracle_band_generate.restype = ctypes.c_int
-        _lib.tdx_oracle_band_generate.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
-    return _lib
-
-
-def itemsize(desc) -> int:
-    from torchdistx_b200 import _cabi as C
-
-    return {C.TDX_F32: 4, C.TDX_RAW32: 4, C.TDX_RAW64: 8, C.TDX_I64: 8, C.TDX_RAW8: 1}.get(desc.dtype, 2)
-
-
-def generate(desc) -> np.ndarray:
-    """What the kernels write for `desc` (any source the restatements know), as bytes."""
-    out = np.empty(int(desc.elem_count) * itemsize(desc), dtype=np.uint8)
-    rc = oracle().tdx_oracle_band_generate(ctypes.byref(desc), out.ctypes.data_as(ctypes.c_void_p))
-    assert rc == 0, "descriptor outside the oracle's specification"
-    return out
 
 
 def as_tensor(raw: np.ndarray, dtype: torch.dtype) -> torch.Tensor:

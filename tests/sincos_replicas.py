@@ -1,17 +1,10 @@
 """Small replicas of the sinusoidal position tables of transformers 5.5 (the four builders verbatim,
-and the modules that register and re-initialise them), and the CPU restatement of TDX_SRC_SINCOS
-(tests/sincos_oracle.c)."""
-import ctypes
+and the modules that register and re-initialise them)."""
 import math
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 import torch
 from torch import nn
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def sinusoids(length: int, channels: int, max_timescale: float = 10000) -> torch.Tensor:
@@ -116,34 +109,6 @@ class GPTJAttentionPositions(nn.Module):
                              persistent=False)
         with torch.no_grad():
             self.embed_positions.copy_(create_sinusoidal_positions(max_positions, pos_embd_dim))
-
-
-_lib = None
-
-
-def oracle():
-    """tests/sincos_oracle.c, built once per process into a temporary directory."""
-    global _lib
-    if _lib is None:
-        so = os.path.join(tempfile.mkdtemp(prefix="tdx_sincos_oracle_"), "libsincos_oracle.so")
-        subprocess.run(["gcc", "-O2", "-fPIC", "-std=c11", "-ffp-contract=off", "-fno-fast-math", "-shared",
-                        "-I" + os.path.join(ROOT, "include"), "-I" + os.path.join(ROOT, "oracle"),
-                        "-o", so, os.path.join(ROOT, "tests", "sincos_oracle.c"), "-lm"], check=True)
-        _lib = ctypes.CDLL(so)
-        _lib.tdx_oracle_sincos_generate.restype = ctypes.c_int
-        _lib.tdx_oracle_sincos_generate.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
-    return _lib
-
-
-def generate(desc) -> np.ndarray:
-    """What the kernels write for `desc` (any source the restatements know), element bits."""
-    from torchdistx_b200 import _cabi as C
-
-    isz = {C.TDX_F32: 4, C.TDX_RAW32: 4, C.TDX_RAW64: 8, C.TDX_I64: 8, C.TDX_RAW8: 1}.get(desc.dtype, 2)
-    out = np.empty(int(desc.elem_count), dtype={1: np.uint8, 2: np.uint16, 4: np.uint32, 8: np.uint64}[isz])
-    rc = oracle().tdx_oracle_sincos_generate(ctypes.byref(desc), out.ctypes.data_as(ctypes.c_void_p))
-    assert rc == 0, "descriptor outside the oracle's specification"
-    return out
 
 
 def as_tensor(bits: np.ndarray, dtype: torch.dtype) -> torch.Tensor:

@@ -1,17 +1,11 @@
 """Small replicas of the state-space / linear-attention initialisers of transformers 5.5 (the
-classes themselves are not instantiated: their constructors load kernels from the hub), and the
-CPU restatement of the extension's kernels (tests/ssm_oracle.c)."""
-import ctypes
+classes themselves are not instantiated: their constructors load kernels from the hub)."""
 import math
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 import torch
 from torch import nn
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 T_MIN, T_MAX, FLOOR = 0.001, 0.1, 1e-4
 
 
@@ -80,34 +74,6 @@ class Buffers(nn.Module):
 
 def inv_softplus(x: float) -> float:
     return x + math.log(-math.expm1(-x))
-
-
-_lib = None
-
-
-def oracle():
-    """tests/ssm_oracle.c, built once per process into a temporary directory."""
-    global _lib
-    if _lib is None:
-        so = os.path.join(tempfile.mkdtemp(prefix="tdx_ssm_oracle_"), "libssm_oracle.so")
-        subprocess.run(["gcc", "-O2", "-fPIC", "-std=c11", "-ffp-contract=off", "-fno-fast-math", "-shared",
-                        "-I" + os.path.join(ROOT, "include"), "-I" + os.path.join(ROOT, "oracle"),
-                        "-o", so, os.path.join(ROOT, "tests", "ssm_oracle.c"), "-lm"], check=True)
-        _lib = ctypes.CDLL(so)
-        _lib.tdx_oracle_ssm_generate.restype = ctypes.c_int
-        _lib.tdx_oracle_ssm_generate.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
-    return _lib
-
-
-def generate(desc) -> np.ndarray:
-    """What the kernels write for `desc`, element bits as a numpy array."""
-    from torchdistx_b200 import _cabi as C
-
-    isz = {C.TDX_F32: 4, C.TDX_RAW32: 4, C.TDX_RAW64: 8, C.TDX_I64: 8, C.TDX_RAW8: 1}.get(desc.dtype, 2)
-    out = np.empty(int(desc.elem_count), dtype={1: np.uint8, 2: np.uint16, 4: np.uint32, 8: np.uint64}[isz])
-    rc = oracle().tdx_oracle_ssm_generate(ctypes.byref(desc), out.ctypes.data_as(ctypes.c_void_p))
-    assert rc == 0, "descriptor outside the oracle's specification"
-    return out
 
 
 def as_tensor(bits: np.ndarray, dtype: torch.dtype) -> torch.Tensor:

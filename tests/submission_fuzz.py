@@ -18,8 +18,9 @@ offset of the destination in one arena.  Destinations are packed back to back at
 share 16-byte lines.  Copies read a staged source buffer of their own.
 
 `route(specs)` restates the routing -- family_of, the table threshold and the twin fallback, the rider
-rule -- and gives the kernel family of every descriptor; `launches(specs)` the launch count that follows.
-Nothing here needs a GPU.
+rule -- and gives the kernel family of every descriptor; `launches(specs)` the launch count that follows;
+`oracle_bits(spec, d)` what the CPU restatement holds a descriptor's first elements to.  Nothing here
+needs a GPU.
 """
 from __future__ import annotations
 
@@ -29,6 +30,7 @@ from typing import Dict, List, Optional
 
 import numpy as np
 
+from oracle import tdx_oracle as O
 from torchdistx_b200 import _cabi as C
 
 SM = 132  # the host's assumption without a device (H100 SXM); the GPU tests pass the device's own count
@@ -41,8 +43,7 @@ DIRECT16_TILE_ELEMS = 1024 * 8  # 16-bit direct kernels: 1024 vectors
 STATIC_TILES_PER_CTA = 8
 MAX_TABLE_BYTES = 1 << 30
 
-ISZ = {C.TDX_F32: 4, C.TDX_BF16: 2, C.TDX_F16: 2, C.TDX_I64: 8, C.TDX_RAW8: 1, C.TDX_RAW16: 2, C.TDX_RAW32: 4,
-       C.TDX_RAW64: 8}
+ISZ = C.ITEMSIZE
 U, N = C.TDX_SRC_UNIFORM, C.TDX_SRC_NORMAL
 FLOATS = (C.TDX_F32, C.TDX_BF16, C.TDX_F16)
 WIDE = C.TDX_ALGO_WIDE32
@@ -227,6 +228,22 @@ def alone(spec: Spec) -> Spec:
     if kw["src"] in (U, N) and resolve_algo(kw) not in (C.TDX_ALGO_ATEN, C.TDX_ALGO_ATEN_WIDE):
         kw["algo"] = kw.get("algo", 0) | C.TDX_ALGO_NOLUT
     return replace(spec, kw=kw)
+
+
+def oracle_bits(spec: Spec, d) -> Optional[np.ndarray]:
+    """The restatement's element bits of the first elements of `d` (`spec`'s descriptor, cut short), or
+    None where no bar applies."""
+    kw = spec.kw
+    if is_aten(kw):  # (its unit uniform draws only)
+        if kw["src"] != U or kw["dtype"] != C.TDX_F32 or kw.get("epi") or (kw["p0"], kw["p1"]) != (0.0, 1.0):
+            return None
+        return O.aten_units(d).view(np.uint32)
+    if kw["src"] == C.TDX_SRC_SINCOS or (kw["src"] == N and kw.get("epi")):
+        # (sincos: its restatement's bar grows with the row index -- held bit for bit to ATen's CUDA
+        # construction in tests/test_sincos_tables_gpu.py; a normal through an epilogue carries the
+        # generator's ulp into every step -- held to ATen on the same draws in tests/test_epilogue_aten_gpu.py)
+        return None
+    return O.generate(d)
 
 
 # ---- drawing descriptors ---------------------------------------------------------------------------

@@ -1,6 +1,6 @@
 """ATen's own CUDA stream (`rng="aten"`, TDX_ALGO_ATEN) without a GPU: ATen's launch policy, the C
-restatement tests/aten_stream_oracle.c pinned to curand's own host code, the library's validation of
-the descriptors, and the `rng=` option of the public calls."""
+restatement oracle/tdx_philox.c pinned to curand's own host code, the library's validation of the
+descriptors, and the `rng=` option of the public calls."""
 import ctypes
 import os
 import shutil
@@ -13,7 +13,7 @@ from torchdistx_b200 import _C
 from torchdistx_b200 import _cabi as C
 from torchdistx_b200.deferred_init import deferred_init, materialize_module, materialize_tensor
 
-HERE = os.path.dirname(os.path.abspath(__file__))
+ORACLE = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle")
 CUDA_INCLUDE = "/usr/local/cuda/include"
 
 
@@ -37,7 +37,7 @@ HARNESS = r"""
 #include <cmath>
 #include <curand_kernel.h>
 extern "C" {
-#include "aten_stream_oracle.c"
+#include "tdx_philox.c"
 }
 int main() {
   const unsigned long long seeds[3] = {0ull, 42ull, 0x123456789abcdefull};
@@ -81,7 +81,7 @@ def test_oracle_is_curand(tmp_path):
     src = tmp_path / "h.cc"
     src.write_text(HARNESS)
     exe = tmp_path / "h"
-    subprocess.run(["g++", "-O2", "-mfma", "-ffp-contract=fast", "-I", CUDA_INCLUDE, "-I", HERE, str(src), "-o", str(exe)],
+    subprocess.run(["g++", "-O2", "-mfma", "-ffp-contract=fast", "-I", CUDA_INCLUDE, "-I", ORACLE, str(src), "-o", str(exe)],
                    check=True, capture_output=True)
     n, bad_word, bad_uniform, bad_normal = map(int, subprocess.run([str(exe)], check=True, capture_output=True,
                                                                    text=True).stdout.split())

@@ -1,7 +1,7 @@
 """Causal-mask buffers (TDX_SRC_BAND) without a GPU: planner verdicts on the real transformers classes,
 the programs that stay opaque, InitPlan for models that could not be planned before, descriptor
 validation, and the host chain InitPlan -> JSON -> descriptors -> CPU restatement of the kernel
-(tests/band_oracle.c) against the eager CPU construction, whole, in shards and at odd ranges."""
+(oracle/tdx_oracle.c) against the eager CPU construction, whole, in shards and at odd ranges."""
 import json
 import warnings
 
@@ -11,6 +11,7 @@ import transformers as T
 from torch import nn
 
 import band_replicas as R
+from oracle import tdx_oracle as O
 from torchdistx_b200 import _cabi as C
 from torchdistx_b200.deferred_init import deferred_init, materialize_module, plan_report
 from torchdistx_b200.plan import FORMAT, FORMAT_BAND, InitPlan, entry_descriptors
@@ -184,16 +185,6 @@ class Masks(nn.Module):
         self.int64 = nn.Parameter(torch.tril(torch.ones((3, 19, 21), dtype=torch.int64), 3), requires_grad=False)
 
 
-def _eval(plan, shard=None):
-    table, _ = plan.descriptors(7, 0, shard)
-    out = {}
-    for e, sizes, descs in table:
-        dtype = getattr(torch, {"Bool": "bool", "Float": "float32", "BFloat16": "bfloat16", "Long": "int64"}[e.dtype])
-        parts = [R.as_tensor(R.generate(d), dtype) for d in descs]  # (none: a rank past the last chunk)
-        out[e.name] = (torch.cat(parts) if parts else torch.empty(0, dtype=dtype)).reshape(sizes)
-    return out
-
-
 def test_plan_round_trip_and_cpu_restatement(tmp_path):
     m = deferred_init(Masks)
     plan = InitPlan.from_module(m)
@@ -204,13 +195,13 @@ def test_plan_round_trip_and_cpu_restatement(tmp_path):
     plan = InitPlan.load(str(p))
     eager = dict(Masks().named_parameters())
     eager.update(dict(Masks().named_buffers()))
-    got = _eval(plan)
+    got, _, _ = O.evaluate_plan(plan, 7, 0)
     assert set(got) == set(eager)
     for name, want in eager.items():
         assert got[name].dtype == want.dtype and torch.equal(got[name], want.detach()), name
     # parameters in shards: torch.chunk of the whole (a band is indexed by the global element)
     for world in (2, 3, 5):
-        parts = [_eval(plan, shard=(r, world)) for r in range(world)]
+        parts = [O.evaluate_plan(plan, 7, 0, shard=(r, world))[0] for r in range(world)]
         for name in ("wide", "int64"):
             assert torch.equal(torch.cat([q[name] for q in parts]), got[name]), (name, world)
     # odd element ranges of every entry: a range starting mid-row, of any length
@@ -219,5 +210,5 @@ def test_plan_round_trip_and_cpu_restatement(tmp_path):
         flat = eager[e.name].detach().reshape(-1)
         for begin, count in ((1, 7), (13, 29), (flat.numel() - 3, 3), (5, flat.numel() - 9)):
             descs = entry_descriptors(e, 0, begin, count, 7, [])
-            part = torch.cat([R.as_tensor(R.generate(d), dtype) for d in descs])
+            part = torch.cat([R.as_tensor(O.generate(d), dtype) for d in descs])
             assert torch.equal(part, flat[begin:begin + count]), (e.name, begin, count)

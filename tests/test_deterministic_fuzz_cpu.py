@@ -2,8 +2,7 @@
 and host copies (tests/det_programs.py), each with the planner's verdict restated from its rules.
 
 For every seed: the fuse / replay verdict of plan_report against the program's label, then
-InitPlan.from_module -> descriptors -> the CPU restatements of the kernels (tests/band_oracle.c, which
-includes the gather, sincos, state-space and base restatements) against the same program run eagerly on
+InitPlan.from_module -> descriptors -> the CPU restatement of the kernels (oracle/tdx_oracle.c) against the same program run eagerly on
 the CPU.  Bit-exact wherever the kernels do no fp32 arithmetic ATen's CPU kernels do differently: index
 programs without steps, band masks, constants, copies and casts -- and every replayed program, which the
 plan stores by value.  Programs with fp32 steps (ATen's CPU `/` divides where the CUDA kernel multiplies by
@@ -16,9 +15,10 @@ import torch
 
 import band_replicas as R
 import det_programs as D
+from oracle import tdx_oracle as O
 from torchdistx_b200 import _cabi as C
 from torchdistx_b200.deferred_init import deferred_init, plan_report
-from torchdistx_b200.plan import _DTYPES, InitPlan, gather_source, value_tensor
+from torchdistx_b200.plan import InitPlan
 
 SEEDS = 6000  # seeds of the whole file (about a minute on one core)
 CHUNKS = 10
@@ -41,26 +41,6 @@ def verdict_errors(progs, report):
         if not p.fuse and info["fusible"]:
             bad.append(f"{p.name}: label replay, planner fused it as {info['source']}: {p.text}")
     return bad
-
-
-def evaluate(plan, shard=None):
-    """{name: tensor} the descriptor table writes, by the CPU restatements (gather sources staged on the host)."""
-    keep = []
-
-    def host_src(g):
-        keep.append(gather_source(g, torch.uint8).clone())
-        return keep[-1].data_ptr()
-
-    table, _ = plan.descriptors(7, 0, shard, gather_src=host_src)
-    out = {}
-    for e, sizes, descs in table:
-        dtype = _DTYPES[e.dtype]
-        if e.source == "value":
-            out[e.name] = value_tensor(e, shard)
-            continue
-        parts = [R.as_tensor(R.generate(d), dtype) for d in descs]
-        out[e.name] = (torch.cat(parts) if parts else torch.empty(0, dtype=dtype)).reshape(sizes)
-    return out
 
 
 def same_bits(got, want):
@@ -94,7 +74,7 @@ def sincos_close(got, want, p, entry):
     half = seg["sincos_half"]
     col = C.make_desc(0, dtype=C.TDX_F32, src=C.TDX_SRC_IOTA, elem_count=half, p0=seg["p0"], p1=seg["p1"],
                       epi=seg["epilogue"])
-    f_o = R.as_tensor(R.generate(col), torch.float32).double()
+    f_o = R.as_tensor(O.generate(col), torch.float32).double()
     f_e = p.col().double()
     differ = ~((f_o == f_e) | (torch.isnan(f_o) & torch.isnan(f_e)))
     rows = got.shape[0]
@@ -113,7 +93,7 @@ def check_seed(seed, stats):
     m = deferred_init(D.DetModule, progs)
     errors = verdict_errors(progs, plan_report(m))
     plan = InitPlan.from_module(m)
-    got = evaluate(plan)
+    got = O.evaluate_plan(plan, 7, 0)[0]
     eager = dict(list(D.DetModule(progs).named_parameters()) + list(D.DetModule(progs).named_buffers()))
     entries = {e.name: e for e in plan.entries}
     for p in progs:
@@ -149,10 +129,10 @@ def test_shards_of_restated_plans_concatenate_to_the_whole():
         r = random.Random(10_000 + seed)
         progs = D.gen_module(r)
         plan = InitPlan.from_module(deferred_init(D.DetModule, progs))
-        whole = evaluate(plan)
+        whole = O.evaluate_plan(plan, 7, 0)[0]
         kinds = {e.name: e.kind for e in plan.entries}
         for world in (2, 3, 8):
-            parts = [evaluate(plan, shard=(rank, world)) for rank in range(world)]
+            parts = [O.evaluate_plan(plan, 7, 0, shard=(rank, world))[0] for rank in range(world)]
             for name, t in whole.items():
                 if kinds[name] == "param" and t.dim() >= 1:
                     cat = torch.cat([q[name] for q in parts])

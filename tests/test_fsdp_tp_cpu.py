@@ -7,7 +7,7 @@
 - Values through the host chain, per coordinate: the layouts come from a meta model handed to
   ``parallelize_module`` and ``fully_shard`` on one rank of the fake backend; the deferred recording
   goes through InitPlan -> JSON -> ``descriptors(blocks=...)`` -> the CPU restatement
-  (tests/window_oracle.c).  Every block is its chunk steps applied to the unsharded restatement, bit
+  (oracle/tdx_oracle.c).  Every block is its chunk steps applied to the unsharded restatement, bit
   for bit, and the unsharded restatement is the eager constructor's tensor (constants bit-exact, draws
   T1); every rank advances the generator alike.
 - The ValueErrors of ``local_block``, ``init_sharded_module`` and ``blocks=``, and the descriptors of the
@@ -19,7 +19,6 @@ import socket
 import sys
 import tempfile
 
-import numpy as np
 import pytest
 import torch
 import torch.distributed as dist
@@ -27,14 +26,13 @@ import torch.multiprocessing as mp
 from torch import nn
 
 from oracle import cases
-from torchdistx_b200 import _cabi as C
+from oracle import tdx_oracle as O
 from torchdistx_b200.deferred_init import deferred_init
 from torchdistx_b200.parallel import local_block, tp_placements
-from torchdistx_b200.plan import _DTYPES, InitPlan, chunk_steps, gather_source, init_sharded_module, narrowed, \
-    value_tensor
+from torchdistx_b200.plan import InitPlan, chunk_steps, init_sharded_module, narrowed
 
 from test_plan_oracle_cpu import OFFSET, SEED, check_t1, compare_with_eager, named, plan_of
-from test_tp_shard_cpu import COPIES_ARGS, COPIES_PLAN, LLAMA_PLAN, OPT_PLAN, Copies, Geometry, evaluate, oracle
+from test_tp_shard_cpu import COPIES_ARGS, COPIES_PLAN, LLAMA_PLAN, OPT_PLAN, Copies, Geometry
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 MESHES = {"dp2_tp4": (2, 4), "dp4_tp2": (4, 2), "hsdp_2x2_tp2": (2, 2, 2)}
@@ -226,7 +224,7 @@ def check_coordinates(plan, per_rank, whole, end, own=None):
     windows = 0
     entries = {e.name: e for e in plan.entries}
     for blocks in per_rank:
-        got, e_end, w = evaluate_blocks(plan, blocks)
+        got, e_end, w = O.evaluate_plan(plan, SEED, OFFSET, blocks=blocks)
         assert e_end == end  # (global sizes only: every rank advances the generator alike)
         windows += w
         for name, steps in blocks.items():
@@ -240,45 +238,6 @@ def check_coordinates(plan, per_rank, whole, end, own=None):
     return windows
 
 
-def evaluate_blocks(plan, blocks):
-    """({name: tensor}, generator offset after, windowed descriptors) of what `descriptors(blocks=...)`
-    writes, by the restatement; entries listed whole are narrowed here, as InitPlan.materialize does."""
-    keep = []  # (the sources of copy segments, staged in host memory)
-
-    def host_src(g):
-        keep.append(gather_source(g, torch.uint8).clone())
-        return keep[-1].data_ptr()
-
-    table, end = plan.descriptors(SEED, OFFSET, gather_src=host_src, blocks=blocks)
-    out, windows = {}, 0
-    for e, sizes, descs in table:
-        steps = blocks.get(e.name, [])
-        if e.source == "alias":
-            out[e.name] = out[e.alias_of]
-            continue
-        if e.source == "value":
-            out[e.name] = value_tensor(e, steps=steps)
-            assert torch.equal(out[e.name], apply_steps(value_tensor(e), steps))
-            continue
-        dtype = _DTYPES[e.dtype]
-        isz = torch.empty((), dtype=dtype).element_size()
-        numel = int(np.prod(sizes)) if sizes else 1
-        buf = np.zeros(numel * isz, dtype=np.uint8)
-        covered = 0
-        for d in descs:
-            part = np.empty(int(d.elem_count) * isz, dtype=np.uint8)
-            assert oracle().tdx_oracle_window_generate(ctypes.byref(d), part.ctypes.data_as(ctypes.c_void_p)) == 0
-            at = int(d.dst or 0)
-            buf[at: at + part.size] = part
-            covered += int(d.elem_count)
-            windows += bool(d.reserved & C.TDX_FLAG_WINDOW)
-        assert covered == numel, (e.name, covered, numel)  # the descriptors tile the block
-        out[e.name] = torch.from_numpy(buf).view(dtype).reshape(sizes) if numel else torch.empty(sizes, dtype=dtype)
-        if narrowed(e, steps=steps):
-            out[e.name] = apply_steps(out[e.name], steps).contiguous()
-    return out, end, windows
-
-
 @pytest.mark.parametrize("case", ["llama_v11_h12", "opt_v11_h12", "tiny_llama", "family_opt"])
 @pytest.mark.parametrize("mesh", list(MESHES))
 def test_blocks_through_the_host_chain_per_coordinate(case, mesh, tmp_path):
@@ -286,7 +245,7 @@ def test_blocks_through_the_host_chain_per_coordinate(case, mesh, tmp_path):
     plan = InitPlan.from_module(deferred_init(lambda: built(fn)))
     plan.save(str(tmp_path / "p.json"))
     plan = InitPlan.load(str(tmp_path / "p.json"))
-    whole, end, _ = evaluate(plan)
+    whole, end, _ = O.evaluate_plan(plan, SEED, OFFSET)
     torch.manual_seed(SEED)
     own = named(built(fn))
     compare_with_eager(plan, whole, own, own)  # the unsharded restatement is the eager model
@@ -306,7 +265,7 @@ def test_three_dims_and_dim_0_rows_of_every_window(dtype, tmp_path):
     plan = InitPlan.from_module(deferred_init(lambda: Geometry().to(dtype)))
     plan.save(str(tmp_path / "p.json"))
     plan = InitPlan.load(str(tmp_path / "p.json"))
-    whole, end, _ = evaluate(plan)
+    whole, end, _ = O.evaluate_plan(plan, SEED, OFFSET)
     for dp, tp in ((2, 4), (3, 2), (4, 3)):
         per_rank = [{"w3": [(0, d, dp), (2, t, tp)], "u": [(0, d, dp), (1, t, tp)], "tn": [(0, t, tp), (0, d, dp)]}
                     for d in range(dp) for t in range(tp)]
@@ -319,7 +278,7 @@ def test_copy_programs_are_built_whole_and_narrowed_on_both_dims(dtype):
     fn = lambda: Copies(*args, cases.DTYPES[dtype])
     torch.manual_seed(0)
     plan = InitPlan.from_module(deferred_init(fn))
-    whole, end, _ = evaluate(plan)
+    whole, end, _ = O.evaluate_plan(plan, SEED, OFFSET)
     torch.manual_seed(0)
     eager_model = fn()
     for k in ("pos.weight", "lin.weight"):  # (copies: bit for bit)

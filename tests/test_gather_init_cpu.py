@@ -1,12 +1,8 @@
 """Copies of host-built tensors (TDX_SRC_GATHER) without a GPU: planner verdicts on the real Pegasus,
 Marian and RWKV classes, the negatives that stay opaque, the version check, descriptor validation, and
-the host chain InitPlan -> JSON -> descriptors -> CPU restatement (tests/gather_oracle.c) against the
+the host chain InitPlan -> JSON -> descriptors -> CPU restatement (oracle/tdx_oracle.c) against the
 eager CPU construction, whole and in shards."""
-import ctypes
 import json
-import os
-import subprocess
-import tempfile
 import warnings
 
 import numpy as np
@@ -15,13 +11,13 @@ import torch
 import transformers as T
 from torch import nn
 
+from oracle import tdx_oracle as O
 from torchdistx_b200 import _C
 from torchdistx_b200 import _cabi as C
 from torchdistx_b200.deferred_init import deferred_init, materialize_tensor, plan_report
-from torchdistx_b200.plan import FORMAT_GATHER, InitPlan, gather_source
+from torchdistx_b200.plan import FORMAT_GATHER, InitPlan
 
 warnings.filterwarnings("ignore", module="transformers")
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 _ENC_DEC = dict(vocab_size=64, d_model=32, encoder_layers=1, decoder_layers=1, encoder_attention_heads=2,
                 decoder_attention_heads=2, encoder_ffn_dim=64, decoder_ffn_dim=64, max_position_embeddings=50)
@@ -152,51 +148,6 @@ def test_library_validates_the_gather_descriptor():
             C.prepare([d])
 
 
-_lib = None
-
-
-def oracle():
-    """tests/gather_oracle.c, built once per process into a temporary directory."""
-    global _lib
-    if _lib is None:
-        so = os.path.join(tempfile.mkdtemp(prefix="tdx_gather_oracle_"), "libgather_oracle.so")
-        subprocess.run(["gcc", "-O2", "-fPIC", "-std=c11", "-ffp-contract=off", "-fno-fast-math", "-shared",
-                        "-I" + os.path.join(ROOT, "include"), "-I" + os.path.join(ROOT, "oracle"),
-                        "-I" + os.path.join(ROOT, "tests"), "-o", so,
-                        os.path.join(ROOT, "tests", "gather_oracle.c"), "-lm"], check=True)
-        _lib = ctypes.CDLL(so)
-        _lib.tdx_oracle_gather_generate.restype = ctypes.c_int
-        _lib.tdx_oracle_gather_generate.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
-    return _lib
-
-
-_DT = {"Float": torch.float32, "BFloat16": torch.bfloat16, "Half": torch.float16, "Long": torch.int64}
-
-
-def _eval(plan, shard=None):
-    """Every gather entry of the plan through the restatement (the sources staged in host memory)."""
-    keep = []
-
-    def host_src(g):
-        keep.append(gather_source(g, torch.uint8).clone())
-        return keep[-1].data_ptr()
-
-    table, _ = plan.descriptors(7, 0, shard, gather_src=host_src)
-    out = {}
-    for e, sizes, descs in table:
-        if not any(g["source"] == "gather" for g in e.segments):
-            continue
-        dtype = _DT[e.dtype]
-        parts = []
-        for d in descs:
-            isz = torch.empty((), dtype=dtype).element_size()
-            buf = np.empty(int(d.elem_count) * isz, dtype=np.uint8)
-            assert oracle().tdx_oracle_gather_generate(ctypes.byref(d), buf.ctypes.data_as(ctypes.c_void_p)) == 0
-            parts.append(torch.from_numpy(buf).view(dtype))
-        out[e.name] = torch.cat(parts).reshape(sizes)
-    return out
-
-
 class Steps(nn.Module):
     """Gather segments with a padding row, an epilogue and a broadcast source, in `dtype` from the start
     (steps on a 16-bit tensor round after each; the scalars are exact in every dtype, because ATen's
@@ -230,7 +181,8 @@ def test_plan_round_trip_and_cpu_restatement(tmp_path, dtype):
     plan.save(str(p))
     assert json.load(open(p))["format"] == FORMAT_GATHER and plan.uses_gather()
     plan = InitPlan.load(str(p))
-    got = _eval(plan)
+    whole, _, _ = O.evaluate_plan(plan, 7, 0)
+    got = {e.name: whole[e.name] for e in plan.entries if any(g["source"] == "gather" for g in e.segments)}
     torch.manual_seed(0)
     both = Both(table, row, dtype)
     eager = {f"peg.{t}": dict(both.peg.named_parameters())[t] for t in TABLES}
@@ -242,7 +194,7 @@ def test_plan_round_trip_and_cpu_restatement(tmp_path, dtype):
         assert torch.equal(got[name].view(torch.uint8), want.contiguous().view(torch.uint8)), (name, dtype)
     # shards of the parameters are torch.chunk of the whole (61 and 37 rows: ragged)
     for world in (2, 3, 8):
-        parts = [_eval(plan, shard=(r, world)) for r in range(world)]
+        parts = [O.evaluate_plan(plan, 7, 0, shard=(r, world))[0] for r in range(world)]
         for name, whole in got.items():
             cat = torch.cat([q[name] for q in parts])
             assert torch.equal(cat.view(torch.uint8), whole.view(torch.uint8)), (world, name)

@@ -8,9 +8,8 @@ included.  For every cut:
     needs (laid out by tdx_init_prepare);
   * each piece sits at its destination's address mod 16;
   * on tables shrunk to a few thousand elements per descriptor, the pieces' descriptors, evaluated by the
-    C restatements (tests/band_oracle.c with the plain generators, index programs, sinusoid tables,
-    state-space steps and copies it includes, tests/window_oracle.c for windows, ATen's stream through
-    tests/aten_stream_oracle.c) and concatenated, equal the uncut descriptor byte for byte.
+    C restatement (oracle/tdx_oracle.c; ATen's stream: its unit draws) and concatenated, equal the uncut
+    descriptor byte for byte.
 """
 import ctypes
 import os
@@ -22,9 +21,7 @@ import pytest
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 import submission_fuzz as F  # noqa: E402
-from band_replicas import generate as band_generate  # noqa: E402
-from test_plan_aten_cpu import draws as aten_draws  # noqa: E402
-from test_tp_shard_cpu import oracle as window_oracle  # noqa: E402
+from oracle import tdx_oracle as O  # noqa: E402
 from torchdistx_b200 import _cabi as C  # noqa: E402
 
 HOST = 0x7F00_0000_0000  # where the fake host arena starts (16-byte aligned; nothing is written there)
@@ -84,23 +81,9 @@ def test_the_cut_of_every_fuzz_table(seed):
             assert passes >= -(-total // staging)
 
 
-def evaluate(d, host_source):
-    """What the kernels write for descriptor `d` (ATen's stream: the unit draws of its global elements)."""
-    n = int(d.elem_count)
-    if F.is_aten(dict(algo=int(d.algo))):
-        i = np.arange(n, dtype=np.int64)
-        if d.reserved & C.TDX_FLAG_WINDOW:
-            W, P = int(d.fill_bits[0]) & 0xFFFFFFFF, int(d.fill_bits[0]) >> 32
-            g = int(d.elem_begin) + (i // W) * P + i % W
-        else:
-            g = int(d.elem_begin) + i
-        return aten_draws(int(d.philox_seed), int(d.philox_offset), int(d.fill_bits[1]), d.src == C.TDX_SRC_NORMAL,
-                          g).view(np.uint8)
-    if d.reserved & C.TDX_FLAG_WINDOW:
-        out = np.empty(n * F.ISZ[d.dtype], dtype=np.uint8)
-        assert window_oracle().tdx_oracle_window_generate(ctypes.byref(d), out.ctypes.data_as(ctypes.c_void_p)) == 0
-        return out
-    return band_generate(d)
+def evaluate(d):
+    """What the kernels write for descriptor `d`, as bytes (ATen's stream: the unit draws of its elements)."""
+    return (O.aten_units(d) if F.is_aten(dict(algo=int(d.algo))) else O.generate(d)).view(np.uint8)
 
 
 def shrunk(seed):
@@ -126,7 +109,7 @@ def test_pieces_evaluate_to_their_uncut_descriptors(seed):
     for t in shrunk(seed):
         host_source = r.integers(0, 256, t.source_bytes, dtype=np.uint8)
         descs = t.descs(HOST, host_source.ctypes.data)
-        whole = [evaluate(d, host_source) for d in descs]
+        whole = [evaluate(d) for d in descs]
         small = min_staging(descs)
         for staging in (small, small + 16, small + 37, small + 4096 + 5, 1 << 20):
             pieces, _ = check_cut(descs, staging)
@@ -143,7 +126,7 @@ def test_pieces_evaluate_to_their_uncut_descriptors(seed):
                         assert getattr(x, k) == getattr(d, k), k
                     assert bytes(x.epi) == bytes(d.epi) and (x.algo, x.reserved & ~C.TDX_FLAG_WINDOW) == \
                         (d.algo, d.reserved & ~C.TDX_FLAG_WINDOW)
-                    got[p.desc].append(evaluate(x, host_source))
+                    got[p.desc].append(evaluate(x))
                 assert at == STAGING + p.staging_off + p.elem_count * isz
             for i, (d, w) in enumerate(zip(descs, whole)):
                 cat = np.concatenate(got[i]) if got[i] else np.empty(0, np.uint8)

@@ -15,7 +15,7 @@ Without a device:
     and of a windowed Shard(2) block of a fused-expert weight, through 256 MiB and 1 MiB + 13 of staging:
     the structural checks of tests/test_host_targets_cpu.py, at least ceil(bytes / staging) passes, and
     the first and last 4096 elements of the pieces that hold local elements 2^31 and 2^32, evaluated by
-    the C restatements, equal the uncut descriptor there.
+    the C restatement, equal the uncut descriptor there.
 """
 import ctypes
 import math
@@ -28,7 +28,8 @@ import pytest
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 import submission_fuzz as F  # noqa: E402
-from test_host_targets_cpu import STAGING, check_cut, evaluate  # noqa: E402
+from oracle import tdx_oracle as O  # noqa: E402
+from test_host_targets_cpu import STAGING, check_cut  # noqa: E402
 from torchdistx_b200 import _cabi as C  # noqa: E402
 
 U, N = F.U, F.N
@@ -327,7 +328,7 @@ def sub_desc(d, x, k):
 def evaluate_sub(d, x, k):
     e, skip = sub_desc(d, x, k)
     isz = F.ISZ[d.dtype]
-    return evaluate(e, None)[skip * isz:]
+    return O.generate(e).view(np.uint8)[skip * isz:]
 
 
 def check_pieces_at_large_offsets(descs, staging):

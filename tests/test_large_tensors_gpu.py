@@ -12,7 +12,7 @@ size allows, with an unaligned start and destination) is:
     pieces are the host cut's own (tdx_init_host_piece_descs: a partial first run, whole runs windowed, a
     partial last run);
   * (b) held at local elements 0, 2^31 - 2048, the elements holding bytes 2^31 and 2^32, and the last 4096
-    elements, to the C restatements under the bars of tests/test_submission_fuzz_gpu.py (check_anchor),
+    elements, to the C restatement under the bars of tests/test_submission_fuzz_gpu.py (check_anchor),
     and the 16-bit generators without an epilogue also to the float64 value of each element's Philox
     half-word (tests/generator_domain.py).
 Then one mixed table of three descriptors past 2^31 elements and small riders, in one submission; ATen's
@@ -37,7 +37,7 @@ import generator_domain as G  # noqa: E402
 import philox_torch as PT  # noqa: E402
 import submission_fuzz as F  # noqa: E402
 import test_large_tensors_cpu as L  # noqa: E402
-from test_submission_fuzz_gpu import check_anchor, oracle_bits  # noqa: E402
+from test_submission_fuzz_gpu import check_anchor  # noqa: E402
 from torchdistx_b200 import _cabi as C  # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -159,14 +159,14 @@ def generator_f64(case, kw, d, x, got):
 
 
 def check_anchors(case, d, big, base_off, host_source, name):
-    """Reference (b): the C restatements at the anchors."""
+    """Reference (b): the C restatement at the anchors."""
     isz, count, kw = case.isz, int(d.elem_count), case.spec.kw
     for x in anchors(count, base_off % 16, isz):
         k = min(ANCHOR, count - x)
         sub, skip = L.sub_desc(d, x, k)
         if sub.src == C.TDX_SRC_GATHER:
             sub.fill_bits[0] = host_source.ctypes.data
-        want = oracle_bits(case.spec, sub)
+        want = F.oracle_bits(case.spec, sub)
         got = big[base_off + x * isz: base_off + (x + k) * isz].cpu().numpy().view(NP_BITS[isz])
         if want is not None:
             check_anchor(Anchored(f"{name} at local element {x}"), case.spec, got, want[skip:])

@@ -4,15 +4,11 @@
 - The draw dtype: a model built in fp32 and cast to bf16 draws every cast parameter on fp32
   (`aten_wide`), which the default stream's `wide` does not record.
 - The descriptor table, `descriptors(..., device_props=(132, 2048))`, evaluated with the C restatement of
-  ATen's stream (tests/aten_stream_oracle.c). It must equal the restatement of each whole draw, cut to
+  ATen's stream (oracle/tdx_oracle.c). It must equal the restatement of each whole draw, cut to
   every rank's block, under `shard=`, tensor-parallel `placements=` and FSDP2 x TP `blocks=`. The generator
   must end at the sum of ATen's increments.
 - Refusals: random programs ATen's stream cannot take, and a table asked for without device properties."""
-import ctypes
 import json
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
@@ -20,6 +16,7 @@ import torch
 from torch import nn
 
 from oracle import cases
+from oracle import tdx_oracle as O
 from torchdistx_b200 import _C
 from torchdistx_b200 import _cabi as C
 from torchdistx_b200.deferred_init import deferred_init
@@ -30,7 +27,6 @@ from test_aten_stream_cpu import policy
 from test_fsdp_tp_cpu import MESHES, apply_steps, fake_blocks
 from test_tp_shard_cpu import MODELS as TP_PLANS
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 H100 = (132, 2048)  # (multiprocessor count, max threads per multiprocessor)
 SEED, OFFSET = 1234, 40
 ROUND_TRIP = [("tiny_llama", "bf16"), ("tiny_llama", "fp32"), ("init_zoo", "fp32"), ("tiny_gpt2", "fp32"),
@@ -136,38 +132,6 @@ def test_a_llama_cast_to_bf16_draws_on_fp32():
 
 
 # ------------------------------------------------------------------------------ the descriptor table
-_lib = None
-
-
-def restatement():
-    """tests/aten_stream_oracle.c with a loop over elements, built once per process."""
-    global _lib
-    if _lib is None:
-        d = tempfile.mkdtemp(prefix="tdx_aten_plan_oracle_")
-        src, so = os.path.join(d, "draws.c"), os.path.join(d, "libdraws.so")
-        with open(src, "w") as f:
-            f.write('#include "aten_stream_oracle.c"\n'
-                    "void aten_draws(uint64_t seed, uint64_t offset, uint32_t S, int normal, const int64_t* g, long n,\n"
-                    "                float* out) {\n"
-                    "  for (long i = 0; i < n; ++i)\n"
-                    "    out[i] = normal ? aten_normal01(seed, offset, S, (uint32_t)g[i]) : aten_uniform01(seed, offset, S,\n"
-                    "                                                                                   (uint32_t)g[i]);\n"
-                    "}\n")
-        subprocess.run(["gcc", "-O2", "-fPIC", "-shared", "-std=c11", "-I", HERE, "-o", so, src, "-lm"], check=True)
-        _lib = ctypes.CDLL(so)
-        _lib.aten_draws.restype = None
-        _lib.aten_draws.argtypes = [ctypes.c_uint64, ctypes.c_uint64, ctypes.c_uint32, ctypes.c_int, ctypes.c_void_p,
-                                    ctypes.c_long, ctypes.c_void_p]
-    return _lib
-
-
-def draws(seed, offset, S, normal, g):
-    g = np.ascontiguousarray(g, dtype=np.int64)
-    out = np.empty(g.size, dtype=np.float32)
-    restatement().aten_draws(seed, offset, S, int(normal), g.ctypes.data, g.size, out.ctypes.data)
-    return out
-
-
 class Programs:
     """Numbers the draw programs (source, parameters, epilogue, algo) a block's elements come from."""
 
@@ -194,17 +158,10 @@ def table_of(plan, steps_of, programs, **kw):
         for d in descs:
             at = int(d.dst or 0) // isz
             n = int(d.elem_count)
-            if d.reserved & C.TDX_FLAG_WINDOW:
-                W, P = d.fill_bits[0] & 0xFFFFFFFF, d.fill_bits[0] >> 32
-                i = np.arange(n)
-                g = d.elem_begin + (i // W) * P + i % W
-            else:
-                g = d.elem_begin + np.arange(n)
             if d.src in (C.TDX_SRC_UNIFORM, C.TDX_SRC_NORMAL):
                 assert d.algo in (C.TDX_ALGO_ATEN, C.TDX_ALGO_ATEN_WIDE), e.name
-                S = d.fill_bits[1]
-                assert S in {_C.aten_stream_policy(n, *H100)[0] for n in e.rng_numels}, e.name
-                vals[at:at + n] = draws(SEED, d.philox_offset, S, d.src == C.TDX_SRC_NORMAL, g)
+                assert d.fill_bits[1] in {_C.aten_stream_policy(n, *H100)[0] for n in e.rng_numels}, e.name
+                vals[at:at + n] = O.aten_units(d)
                 ids[at:at + n] = programs(d.src, d.p0, d.p1, [(d.epi[k].op, d.epi[k].a, d.epi[k].b) for k in range(d.n_epi)],
                                           d.algo)
             else:
@@ -239,11 +196,12 @@ def whole_draws(plan, programs):
             if not drawn(g):
                 ids[lo:hi] = -1
                 continue
-            S = policy(e.rng_numels[g["rng_pass"]], *H100)[0]
-            normal = g["source"] == "normal"
-            vals[lo:hi] = draws(SEED, offsets[g["rng_pass"]], S, normal, np.arange(lo, hi) - g["origin"])
-            ids[lo:hi] = programs(C.TDX_SRC_NORMAL if normal else C.TDX_SRC_UNIFORM, g["p0"], g["p1"], g["epilogue"],
-                                  C.TDX_ALGO_ATEN_WIDE if g["aten_wide"] else C.TDX_ALGO_ATEN)
+            src = C.TDX_SRC_NORMAL if g["source"] == "normal" else C.TDX_SRC_UNIFORM
+            algo = C.TDX_ALGO_ATEN_WIDE if g["aten_wide"] else C.TDX_ALGO_ATEN
+            vals[lo:hi] = O.aten_units(C.make_desc(0, dtype=C.TDX_F32, src=src, elem_begin=lo - g["origin"],
+                                                   elem_count=hi - lo, seed=SEED, offset=offsets[g["rng_pass"]],
+                                                   algo=algo, aten_stride=policy(e.rng_numels[g["rng_pass"]], *H100)[0]))
+            ids[lo:hi] = programs(src, g["p0"], g["p1"], g["epilogue"], algo)
         out[e.name] = (vals.reshape(e.sizes), ids.reshape(e.sizes))
     return out, offset
 

@@ -17,14 +17,13 @@ to the dtype (tests/test_t1_fullsize_gpu.py explains why not with ATen's own bf1
 """
 import math
 
-import numpy as np
 import pytest
 import torch
 
 from oracle import cases
 from oracle import tdx_oracle as O
 from torchdistx_b200.deferred_init import deferred_init
-from torchdistx_b200.plan import InitPlan, offset_increment, value_tensor
+from torchdistx_b200.plan import InitPlan, offset_increment
 
 SEED, OFFSET = 1234, 40
 
@@ -45,38 +44,6 @@ def plan_of(case, dtype, tmp_path=None, post=None):
         plan.save(path)
         plan = InitPlan.load(path)
     return plan
-
-
-def evaluate(plan, shard=None, seed=SEED, offset=OFFSET):
-    """{name: torch tensor} of what the descriptor table writes, by the CPU restatement."""
-    from torchdistx_b200.plan import _DTYPES
-
-    table, end = plan.descriptors(seed, offset, shard)
-    out = {}
-    for e, sizes, descs in table:
-        if e.source == "alias":
-            out[e.name] = out[e.alias_of]
-            continue
-        dtype = _DTYPES[e.dtype]
-        if e.source == "value":
-            out[e.name] = value_tensor(e, shard)
-            assert list(out[e.name].shape) == sizes
-            continue
-        numel = int(np.prod(sizes)) if sizes else 1
-        isz = torch.empty((), dtype=dtype).element_size()
-        buf = np.zeros(numel * isz, dtype=np.uint8)
-        covered = 0
-        for d in descs:
-            got = O.generate(d).view(np.uint8)
-            at = int(d.dst or 0)  # (byte offset inside the tensor; ctypes reads address 0 back as None)
-            assert got.size == d.elem_count * isz and at % isz == 0 and at + got.size <= buf.size, e.name
-            buf[at: at + got.size] = got
-            covered += int(d.elem_count)
-        if e.source != "uninit" and not any(g["source"] == "uninit" for g in e.segment_list()):
-            assert covered == numel, (e.name, covered, numel)  # the segments tile the tensor
-        # (a trailing rank of an uneven split owns no rows)
-        out[e.name] = torch.from_numpy(buf).view(dtype).reshape(sizes) if numel else torch.empty(sizes, dtype=dtype)
-    return out, end
 
 
 def check_t1(name, x, ref, sixteen_bit, moments=True, scale=1.0, alpha=1e-3):
@@ -176,7 +143,7 @@ def compare_with_eager(plan, got, own, wide, skip=(), clamps_by_ks_only=False, s
                                         ("torch_transformer", "fp32")])
 def test_descriptor_table_reproduces_the_eager_constructor(case, dtype, tmp_path):
     plan = plan_of(case, dtype, tmp_path)
-    got, end = evaluate(plan)
+    got, end, _ = O.evaluate_plan(plan, SEED, OFFSET)
     own, wide = eager(case, dtype)
     assert {e.name for e in plan.entries} == set(own)
     n_rng, n_const, n_iota = compare_with_eager(plan, got, own, wide)
@@ -191,7 +158,7 @@ def test_descriptor_table_reproduces_the_eager_constructor(case, dtype, tmp_path
 
 def test_trunc_normal_stays_inside_its_bounds_and_casts_fold():
     plan = plan_of("init_zoo", "fp32")
-    got, _ = evaluate(plan)
+    got = O.evaluate_plan(plan, SEED, OFFSET)[0]
     # nn.init.trunc_normal_(mean=0.1, std=0.02, a=-0.04, b=0.06): uniform -> erfinv -> mul -> add -> clamp;
     # the window ends two sigma BELOW the mean, so the mass piles up under b
     t = got["trunc"]
@@ -199,7 +166,7 @@ def test_trunc_normal_stays_inside_its_bounds_and_casts_fold():
     # Module.to(bf16) after an fp32 construction: the native 16-bit stream where nothing can tell,
     # the fp32 stream rounded (TDX_ALGO_WIDE32) where a second tensor must agree with the first
     plan = plan_of("cast_variant", "fp32")
-    got, _ = evaluate(plan)
+    got = O.evaluate_plan(plan, SEED, OFFSET)[0]
     e = {x.name: x for x in plan.entries}
     assert e["b"].wide and not e["a"].wide and got["b"].dtype == torch.bfloat16
     assert torch.equal(got["b"], got["a"].to(torch.bfloat16))  # `b = a.to(bf16)`: bit for bit
@@ -210,7 +177,7 @@ def test_trunc_normal_stays_inside_its_bounds_and_casts_fold():
 def test_rotary_buffers_of_a_converted_model():
     post = lambda m: m.to(torch.bfloat16)
     plan = plan_of("tiny_llama", "fp32", post=post)
-    got, _ = evaluate(plan)
+    got = O.evaluate_plan(plan, SEED, OFFSET)[0]
     own, _ = eager("tiny_llama", "fp32", post=post)
     for name in ("model.rotary_emb.inv_freq", "model.rotary_emb.original_inv_freq"):
         assert got[name].dtype == torch.bfloat16
@@ -221,7 +188,7 @@ def test_rotary_buffers_of_a_converted_model():
 
 def test_clones_share_their_sources_stream():
     plan = plan_of("clones", "fp32")
-    got, end = evaluate(plan)
+    got, end, _ = O.evaluate_plan(plan, SEED, OFFSET)
     own, _ = eager("clones", "fp32")
     by_pass = {}
     for e in plan.entries:
@@ -239,10 +206,10 @@ def test_clones_share_their_sources_stream():
 @pytest.mark.parametrize("case,dtype", [("tiny_llama", "bf16"), ("padded_embeddings", "fp32"), ("init_zoo", "fp32")])
 def test_shards_concatenate_to_the_whole_and_agree_on_the_generator(case, dtype):
     plan = plan_of(case, dtype)
-    full, end = evaluate(plan)
+    full, end, _ = O.evaluate_plan(plan, SEED, OFFSET)
     kinds = {e.name: e.kind for e in plan.entries}
     for world in (2, 3, 8):
-        parts = [evaluate(plan, shard=(r, world)) for r in range(world)]
+        parts = [O.evaluate_plan(plan, SEED, OFFSET, shard=(r, world))[:2] for r in range(world)]
         assert all(p[1] == end for p in parts)  # every rank advances its generator identically
         for name, t in full.items():
             if kinds[name] == "param" and t.dim() >= 1:
@@ -258,10 +225,10 @@ def test_shards_concatenate_to_the_whole_and_agree_on_the_generator(case, dtype)
 
 def test_seed_and_offset_select_the_stream():
     plan = plan_of("mlp_stack", "fp32")
-    a, _ = evaluate(plan)
-    b, _ = evaluate(plan)
-    c, _ = evaluate(plan, seed=SEED + 1)
-    d, _ = evaluate(plan, offset=OFFSET + 4)
+    a = O.evaluate_plan(plan, SEED, OFFSET)[0]
+    b = O.evaluate_plan(plan, SEED, OFFSET)[0]
+    c = O.evaluate_plan(plan, SEED + 1, OFFSET)[0]
+    d = O.evaluate_plan(plan, SEED, OFFSET + 4)[0]
     w = next(e.name for e in plan.entries if e.source in ("uniform", "normal"))
     assert torch.equal(a[w], b[w]) and not torch.equal(a[w], c[w]) and not torch.equal(a[w], d[w])
 
@@ -282,10 +249,10 @@ def test_a_parameter_stored_by_value_is_chunked_like_the_others():
     plan = InitPlan.from_module(deferred_init(M))
     kinds = {e.name: e.source for e in plan.entries}
     assert kinds["p"] == "value" and kinds["b"] == "value" and kinds["w"] == "normal", kinds
-    full, end = evaluate(plan)
+    full, end, _ = O.evaluate_plan(plan, SEED, OFFSET)
     assert torch.equal(full["p"], torch.tril(torch.ones(7, 4)) * 0.5)
     for world in (2, 3, 8):
-        parts = [evaluate(plan, shard=(r, world)) for r in range(world)]
+        parts = [O.evaluate_plan(plan, SEED, OFFSET, shard=(r, world))[:2] for r in range(world)]
         assert all(e == end for _, e in parts)
         for name in ("p", "w"):
             assert torch.equal(torch.cat([p[name] for p, _ in parts]), full[name]), (name, world)
@@ -302,7 +269,7 @@ def test_model_families_initialise_to_what_their_constructors_compute(family):
     eagerly built model, T0 / T1 (the fuzz tests' x1.5 bounds: ~40 statistical checks per family)."""
     fn = cases.families()[family]
     plan = InitPlan.from_module(deferred_init(fn))
-    got, _ = evaluate(plan)
+    got = O.evaluate_plan(plan, SEED, OFFSET)[0]
     torch.manual_seed(0)
     own = named(fn())
     assert {e.name for e in plan.entries} == set(own)

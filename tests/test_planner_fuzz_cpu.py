@@ -25,6 +25,7 @@ import torch
 from torch import nn
 
 import test_plan_oracle_cpu as T
+from oracle import tdx_oracle as O
 from torchdistx_b200.deferred_init import deferred_init, plan_report
 from torchdistx_b200.plan import InitPlan
 
@@ -43,7 +44,7 @@ def run_seed(seed):
     except ValueError as e:
         assert "random initialisation program the planner cannot fold" in str(e)
         return "replayed"
-    got, _ = T.evaluate(plan)
+    got = O.evaluate_plan(plan, T.SEED, T.OFFSET)[0]
     torch.manual_seed(seed)
     own = T.named(Holder(progs))
     # (a regression net over ~1500 statistical checks, not the parity claim: SURVEY's bounds are 3.5
@@ -78,14 +79,14 @@ def test_writes_through_views_copies_and_shards():
             assert "random initialisation program the planner cannot fold" in str(e)
             seen["replayed"] += 1
             continue
-        got, end = T.evaluate(plan)
+        got, end, _ = O.evaluate_plan(plan, T.SEED, T.OFFSET)
         torch.manual_seed(seed)
         own = T.named(Holder(progs))
         try:
             T.compare_with_eager(plan, got, own, own, clamps_by_ks_only=True, scale=1.5, alpha=1e-6)
         except AssertionError as e:
             raise AssertionError(f"seed {seed}: {e}") from e
-        parts = [T.evaluate(plan, shard=(rank, 3)) for rank in range(3)]
+        parts = [O.evaluate_plan(plan, T.SEED, T.OFFSET, shard=(rank, 3))[:2] for rank in range(3)]
         assert all(p[1] == end for p in parts), seed
         for name, t in got.items():
             cat = torch.cat([p[0][name] for p in parts])
@@ -121,7 +122,7 @@ def test_tensors_derived_from_each_others_intermediate_states():
         except ValueError as e:
             assert "random initialisation program the planner cannot fold" in str(e)
             continue
-        got, _ = T.evaluate(plan)
+        got = O.evaluate_plan(plan, T.SEED, T.OFFSET)[0]
         torch.manual_seed(seed)
         own = T.named(LinkedHolder(progs, links))
         try:
@@ -199,7 +200,7 @@ def test_parameter_data_and_module_idioms():
         except ValueError as e:
             assert "random initialisation program the planner cannot fold" in str(e)
             continue
-        got, _ = T.evaluate(plan)
+        got = O.evaluate_plan(plan, T.SEED, T.OFFSET)[0]
         torch.manual_seed(seed)
         own = T.named(Cell(prog, steps))
         assert plan.entries[0].requires_grad == own["p"].requires_grad, seed
@@ -324,7 +325,7 @@ def test_the_bugs_the_fuzzer_found_stay_fixed():
     for which in ("row_then_all", "slice_only"):
         plan = InitPlan.from_module(deferred_init(shared, which))
         assert plan.entries[0].source == "const" and len(plan.entries[0].segments) == 3
-        got, _ = T.evaluate(plan)
+        got = O.evaluate_plan(plan, T.SEED, T.OFFSET)[0]
         assert torch.equal(got["0"], shared(which)[0].detach()), which
 
     # (b) conversions that have nothing to convert return the tensor itself: still on the fused path

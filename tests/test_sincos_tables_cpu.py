@@ -1,7 +1,7 @@
 """Sinusoidal position tables (Whisper, M2M100 / NLLB, GPT-J, CodeGen, MusicGen) on the fused path,
 without a GPU: planner verdicts on the transformers classes and on replicas of their builders, the
 negatives that stay opaque, InitPlan for models whose tables could not be planned before, and the
-host chain InitPlan -> JSON -> descriptors -> CPU restatement of the kernel (tests/sincos_oracle.c)
+host chain InitPlan -> JSON -> descriptors -> CPU restatement of the kernel (oracle/tdx_oracle.c)
 against the eager CPU construction."""
 import json
 import math
@@ -13,6 +13,7 @@ import transformers as T
 from torch import nn
 
 import sincos_replicas as R
+from oracle import tdx_oracle as O
 from torchdistx_b200 import _cabi as C
 from torchdistx_b200.deferred_init import deferred_init, plan_report
 from torchdistx_b200.plan import FORMAT, FORMAT_SINCOS, InitPlan
@@ -123,15 +124,6 @@ def test_from_module_plans_whisper_and_a_large_m2m100_table():
         assert plan.uses_sincos()
 
 
-def _eval(plan, seed=7, offset=0, shard=None):
-    table, end = plan.descriptors(seed, offset, shard)
-    out = {}
-    for e, sizes, descs in table:
-        dtype = getattr(torch, {"Float": "float32", "BFloat16": "bfloat16", "Half": "float16"}[e.dtype])
-        out[e.name] = torch.cat([R.as_tensor(R.generate(d), dtype) for d in descs]).reshape(sizes) if descs else None
-    return out, end
-
-
 # The column program of each table, run eagerly on the CPU.
 COLUMNS = {
     "whisper.embed_positions.weight": lambda: torch.exp(-(math.log(10000) / 639) * torch.arange(640)),
@@ -152,7 +144,7 @@ def _check(name, entry, got, want):
     half = seg["sincos_half"]
     col = C.make_desc(0, dtype=C.TDX_F32, src=C.TDX_SRC_IOTA, elem_count=half, p0=seg["p0"], p1=seg["p1"],
                       epi=seg["epilogue"])
-    f_o = R.as_tensor(R.generate(col), torch.float32).double()
+    f_o = R.as_tensor(O.generate(col), torch.float32).double()
     f_e = COLUMNS[name]().double()
     differ = f_o != f_e
     assert int(differ.sum()) <= max(1, half // 50), (name, int(differ.sum()))
@@ -176,7 +168,7 @@ def test_plan_round_trip_and_cpu_restatement(tmp_path, dtype):
     plan.save(str(p))
     assert json.load(open(p))["format"] == FORMAT_SINCOS
     plan = InitPlan.load(str(p))
-    got, end = _eval(plan)
+    got, end, _ = O.evaluate_plan(plan, 7, 0)
     eager = {
         "whisper.embed_positions.weight": R.sinusoids(1500, 1280),
         "nllb.weights": R.m2m100_embedding(1026, 1024, 1),
@@ -194,7 +186,7 @@ def test_plan_round_trip_and_cpu_restatement(tmp_path, dtype):
     assert end > 0
     # shards of the parameter are torch.chunk of the whole
     for world in (2, 3, 8):
-        parts = [_eval(plan, shard=(r, world))[0] for r in range(world)]
+        parts = [O.evaluate_plan(plan, 7, 0, shard=(r, world))[0] for r in range(world)]
         whole = torch.cat([q["whisper.embed_positions.weight"] for q in parts])
         assert torch.equal(whole.view(torch.uint8), got["whisper.embed_positions.weight"].view(torch.uint8)), world
 

@@ -1,6 +1,6 @@
 """State-space and linear-attention initialisers (Mamba / Mamba-2 A_log and dt bias, Qwen3-Next's
 random A_log) on the fused path, without a GPU: planner verdicts, the compacted descriptors, and the
-host chain InitPlan -> JSON -> descriptors -> CPU restatement of the kernels (tests/ssm_oracle.c)."""
+host chain InitPlan -> JSON -> descriptors -> CPU restatement of the kernels (oracle/tdx_oracle.c)."""
 import json
 import math
 
@@ -11,6 +11,7 @@ from scipy import stats
 from torch import nn
 
 import ssm_replicas as R
+from oracle import tdx_oracle as O
 from torchdistx_b200 import _cabi as C
 from torchdistx_b200.deferred_init import deferred_init, plan_report
 from torchdistx_b200.plan import FORMAT, FORMAT_SSM, InitPlan, offset_increment
@@ -79,15 +80,6 @@ def test_negatives_stay_opaque():
         assert r[name]["source"] == "opaque" and not r[name]["fusible"], (name, r[name])
 
 
-def _eval(plan, seed, offset, shard=None):
-    table, end = plan.descriptors(seed, offset, shard)
-    out = {}
-    for e, sizes, descs in table:
-        dtype = getattr(torch, {"Float": "float32", "BFloat16": "bfloat16", "Long": "int64"}[e.dtype])
-        out[e.name] = torch.cat([R.as_tensor(R.generate(d), dtype) for d in descs]).reshape(sizes) if descs else None
-    return out, end
-
-
 class Model(nn.Module):
     def __init__(self, heads=4096):
         super().__init__()
@@ -104,7 +96,7 @@ def test_plan_round_trip_and_cpu_restatement(tmp_path):
     assert json.load(open(p))["format"] == FORMAT_SSM
     plan = InitPlan.load(str(p))
     seed, off0 = 1234, 8
-    got, end = _eval(plan, seed, off0)
+    got, end, _ = O.evaluate_plan(plan, seed, off0)
     # generator: Mamba-2's dt draw, Mamba's dead kaiming pass (dt_proj.weight's, then the bias's) and
     # its dt draw, Qwen's dead constructor draw and live _init_weights draw
     n_weight = 96 * 8
@@ -128,9 +120,9 @@ def test_plan_round_trip_and_cpu_restatement(tmp_path):
     assert ks.pvalue > 1e-4, ks
     # shards are torch.chunk of the whole
     for world in (2, 3, 8):
-        parts = [_eval(plan, seed, off0, (r, world))[0] for r in range(world)]
+        parts = [O.evaluate_plan(plan, seed, off0, shard=(r, world))[0] for r in range(world)]
         for name in ("mamba2.A_log", "mamba2.dt_bias", "mamba.A_log", "qwen.A_log", "mamba.dt_proj.bias"):
-            whole = torch.cat([p[name] for p in parts if p[name] is not None and p[name].numel()])
+            whole = torch.cat([p[name] for p in parts if p[name].numel()])
             assert torch.equal(whole.view(-1), got[name].view(-1)), (world, name)
 
 
@@ -150,5 +142,5 @@ def test_make_desc_writes_the_broadcast_geometry():
     d = C.make_desc(0, dtype=C.TDX_F32, src=C.TDX_SRC_IOTA, elem_count=10, p0=1, p1=1, iota_period=5, iota_repeat=2)
     assert list(d.fill_bits) == [5, 2]
     assert list(C.make_desc(0, dtype=C.TDX_F32, src=C.TDX_SRC_IOTA, elem_count=10).fill_bits) == [0, 0]
-    bits = R.generate(d).view(np.float32)
+    bits = O.generate(d).view(np.float32)
     assert bits.tolist() == [1, 1, 2, 2, 3, 3, 4, 4, 5, 5]

@@ -7,6 +7,7 @@ import pytest
 import torch
 
 import ssm_replicas as R
+from oracle import tdx_oracle as O
 from torchdistx_b200 import _C
 from torchdistx_b200 import _cabi as C
 from torchdistx_b200.deferred_init import deferred_init, last_materialize_stats, materialize_module, materialize_tensor
@@ -59,7 +60,7 @@ def test_fused_step_equals_aten_on_the_same_draws(case, dtype):
     # the CPU restatement (C libm): within a few ulp of the libdevice functions -- of the operands where
     # x + log(-expm1(-x)) cancels (|terms| < 10 here)
     head = C.make_desc(0, dtype=d.dtype, src=d.src, elem_count=1 << 14, seed=77, p0=lo, p1=hi, epi=epi)
-    exp_bits = R.as_tensor(R.generate(head), dtype).cuda()
+    exp_bits = R.as_tensor(O.generate(head), dtype).cuda()
     g = got[: 1 << 14]
     cancels = dtype == torch.float32 and case in ("inv_softplus", "dt_chain")
     ok = torch.isclose(g.float(), exp_bits.float(), rtol=4e-6 if dtype == torch.float32 else 1e-2,
@@ -87,8 +88,8 @@ def test_periodic_iota_is_arange_expand_log(begin, count, shift):
     C.submit(ws.data_ptr(), ws.numel())
     torch.cuda.synchronize()
     assert torch.equal(out, cols.view(-1))
-    assert torch.equal(out.cpu(), R.as_tensor(R.generate(d), torch.float32)) or \
-        (out.cpu().view(torch.int32) - R.as_tensor(R.generate(d), torch.float32).view(torch.int32)).abs().max() <= 1
+    assert torch.equal(out.cpu(), R.as_tensor(O.generate(d), torch.float32)) or \
+        (out.cpu().view(torch.int32) - R.as_tensor(O.generate(d), torch.float32).view(torch.int32)).abs().max() <= 1
 
 
 class Model(torch.nn.Module):

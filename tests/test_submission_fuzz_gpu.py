@@ -11,11 +11,10 @@ For every table tests/submission_fuzz.py draws (random mixes and the forced regi
     captured once in a CUDA graph and replayed twice, gives A's bytes every time (each kernel puts its
     work counter back to zero as it leaves).  Tables of more than 47 families go through
     tdx_init_launch three times instead: tdx_plan_upload takes one plan;
-  * a sample of each table's descriptors is anchored to the CPU restatements: tests/window_oracle.c (with
-    the plain generators, index programs and copies it includes; copies read the host copy of their
-    source) and tests/band_oracle.c bit for bit, ATen's stream (tests/aten_stream_oracle.c) for its unit
-    uniform draws, the normals under the bars of tests/test_kernels_gpu.py, erfinv chains within 2 ulp
-    and the state-space steps under the bar of tests/test_ssm_init_cpu.py.
+  * a sample of each table's descriptors is anchored to the CPU restatement (oracle/tdx_oracle.c, through
+    submission_fuzz.oracle_bits; copies read the host copy of their source): bit for bit, ATen's stream
+    for its unit uniform draws, the normals under the bars of tests/test_kernels_gpu.py, erfinv chains
+    within 2 ulp and the state-space steps under the bar of tests/test_ssm_init_cpu.py.
 """
 import ctypes
 import os
@@ -29,16 +28,13 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 import submission_fuzz as F  # noqa: E402
-from band_replicas import generate as band_generate  # noqa: E402
-from test_plan_aten_cpu import draws as aten_draws  # noqa: E402
-from test_tp_shard_cpu import oracle as window_oracle  # noqa: E402
 from torchdistx_b200 import _cabi as C  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
 SEEDS = 120  # (about a minute on one H100)
 CHUNKS = 8
-ANCHORS = 6  # descriptors per table held to the restatements (the first 4096 elements of each)
+ANCHORS = 6  # descriptors per table held to the restatement (the first 4096 elements of each)
 ANCHOR_ELEMS = 4096
 NP_BITS = {1: np.uint8, 2: np.uint16, 4: np.uint32, 8: np.uint64}
 
@@ -77,31 +73,6 @@ def expect_equal(t, got, want, what):
         at = first_diff(got, want)
         n = int((got != want).sum())
         raise AssertionError(f"{t.name}: {what}: {n} bytes differ, first at byte {at} ({owner(t, at)})")
-
-
-def oracle_bits(spec, d):
-    """The restatement's element bits of the first elements of `d`, or None where no bar applies."""
-    kw = spec.kw
-    isz = F.ISZ[kw["dtype"]]
-    if F.is_aten(kw):
-        if kw["src"] != F.U or kw["dtype"] != C.TDX_F32 or kw.get("epi") or (kw["p0"], kw["p1"]) != (0.0, 1.0):
-            return None
-        i = np.arange(d.elem_count, dtype=np.int64)
-        if kw.get("flags", 0) & C.TDX_FLAG_WINDOW:
-            g = d.elem_begin + (i // kw["window_width"]) * kw["window_pitch"] + i % kw["window_width"]
-        else:
-            g = d.elem_begin + i
-        return aten_draws(d.philox_seed, d.philox_offset, int(d.fill_bits[1]), False, g).view(np.uint32)
-    if kw["src"] == C.TDX_SRC_BAND:
-        return band_generate(d).view(NP_BITS[isz])
-    if kw["src"] == C.TDX_SRC_SINCOS or (kw["src"] == F.N and kw.get("epi")):
-        # (sincos: its restatement's bar grows with the row index -- held bit for bit to ATen's CUDA
-        # construction in tests/test_sincos_tables_gpu.py; a normal through an epilogue carries the
-        # generator's ulp into every step -- held to ATen on the same draws in tests/test_epilogue_aten_gpu.py)
-        return None
-    out = np.empty(int(d.elem_count), dtype=NP_BITS[isz])
-    assert window_oracle().tdx_oracle_window_generate(ctypes.byref(d), out.ctypes.data_as(ctypes.c_void_p)) == 0
-    return out
 
 
 def as_f64(bits, dtype):
@@ -161,7 +132,7 @@ def check_anchor(t, spec, got, want):
 
 
 def anchor(t, a, host_source, r):
-    """Holds a sample of the table's descriptors to the restatements; copies read the host copy of their
+    """Holds a sample of the table's descriptors to the restatement; copies read the host copy of their
     staged source."""
     picks = r.choice(len(t.specs), min(ANCHORS, len(t.specs)), replace=False)
     for i in picks:
@@ -170,7 +141,7 @@ def anchor(t, a, host_source, r):
         if n == 0:
             continue
         d = spec.desc(0, host_source.ctypes.data, elem_count=n)
-        want = oracle_bits(spec, d)
+        want = F.oracle_bits(spec, d)
         if want is None:
             continue
         isz = F.ISZ[spec.kw["dtype"]]

@@ -1,16 +1,13 @@
 """Tensor-parallel blocks without a GPU: tiny Llama and OPT recordings through InitPlan -> JSON ->
-descriptors(placements) -> the CPU restatement of windowed descriptors (tests/window_oracle.c).  Every
+descriptors(placements) -> the CPU restatement of windowed descriptors (oracle/tdx_oracle.c).  Every
 rank's Shard(d) block is the rank's torch.chunk of the unsharded restatement, bit for bit, and the
 unsharded restatement is the eager constructor's tensor (constants bit-exact, draws T1); the generator
 advances the same on every rank.  Also: tp_placements against what parallelize_module does on two gloo
 ranks (and materialize_module(parallelize_plan=...) there, by ATen replay), the ValueError cases and the
 library's validation of windowed descriptors."""
-import ctypes
 import os
 import socket
-import subprocess
 import sys
-import tempfile
 import types
 
 import numpy as np
@@ -22,10 +19,11 @@ from torch.distributed.tensor.parallel import (ColwiseParallel, PrepareModuleInp
                                                SequenceParallel)
 
 from oracle import cases
+from oracle import tdx_oracle as O
 from torchdistx_b200 import _cabi as C
 from torchdistx_b200.deferred_init import deferred_init, materialize_module
 from torchdistx_b200.parallel import tp_placements
-from torchdistx_b200.plan import _DTYPES, InitPlan, gather_source, narrowed, value_tensor
+from torchdistx_b200.plan import InitPlan, narrowed
 
 from test_plan_oracle_cpu import OFFSET, SEED, compare_with_eager, eager, plan_of
 
@@ -51,62 +49,6 @@ OPT_PLAN = lambda: {  # (OPT's embedding has a padding row: a constant run insid
 }
 MODELS = {"tiny_llama": LLAMA_PLAN, "family_opt": OPT_PLAN}
 
-_lib = None
-
-
-def oracle():
-    """tests/window_oracle.c, built once per process into a temporary directory."""
-    global _lib
-    if _lib is None:
-        so = os.path.join(tempfile.mkdtemp(prefix="tdx_window_oracle_"), "libwindow_oracle.so")
-        subprocess.run(["gcc", "-O2", "-fPIC", "-std=c11", "-ffp-contract=off", "-fno-fast-math", "-shared",
-                        "-I" + os.path.join(ROOT, "include"), "-I" + os.path.join(ROOT, "oracle"),
-                        "-I" + os.path.join(ROOT, "tests"), "-o", so,
-                        os.path.join(ROOT, "tests", "window_oracle.c"), "-lm"], check=True)
-        _lib = ctypes.CDLL(so)
-        _lib.tdx_oracle_window_generate.restype = ctypes.c_int
-        _lib.tdx_oracle_window_generate.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
-    return _lib
-
-
-def evaluate(plan, shard=None, placements=None):
-    """({name: tensor}, generator offset after) of what the descriptor table writes, by the restatement."""
-    keep = []  # (the sources of copy segments, staged in host memory)
-
-    def host_src(g):
-        keep.append(gather_source(g, torch.uint8).clone())
-        return keep[-1].data_ptr()
-
-    table, end = plan.descriptors(SEED, OFFSET, shard, gather_src=host_src, placements=placements)
-    out, windows = {}, 0
-    for e, sizes, descs in table:
-        if e.source == "alias":
-            out[e.name] = out[e.alias_of]
-            continue
-        dtype = _DTYPES[e.dtype]
-        if e.source == "value":
-            out[e.name] = value_tensor(e, shard, 0 if placements is None else placements.get(e.name))
-            continue
-        isz = torch.empty((), dtype=dtype).element_size()
-        numel = int(np.prod(sizes)) if sizes else 1
-        buf = np.zeros(numel * isz, dtype=np.uint8)
-        covered = 0
-        for d in descs:
-            part = np.empty(int(d.elem_count) * isz, dtype=np.uint8)
-            assert oracle().tdx_oracle_window_generate(ctypes.byref(d), part.ctypes.data_as(ctypes.c_void_p)) == 0
-            at = int(d.dst or 0)
-            buf[at: at + part.size] = part
-            covered += int(d.elem_count)
-            windows += bool(d.reserved & C.TDX_FLAG_WINDOW)
-        assert covered == numel, (e.name, covered, numel)  # the descriptors tile the block
-        # (a trailing rank of an uneven split owns no rows)
-        out[e.name] = torch.from_numpy(buf).view(dtype).reshape(sizes) if numel else torch.empty(sizes, dtype=dtype)
-        dim = None if placements is None else placements.get(e.name)
-        if narrowed(e, shard, dim):  # (listed whole: this rank narrows it, as InitPlan.materialize does)
-            out[e.name] = block(out[e.name], shard[1], shard[0], dim).contiguous()
-    return out, end, windows
-
-
 def block(whole, world, rank, dim):
     """Rank `rank`'s torch.chunk(whole, world, dim) (empty for trailing ranks without rows)."""
     if dim is None:
@@ -120,7 +62,7 @@ def check_blocks(plan, placements, whole, end, worlds=(2, 3, 8)):
     n_windows = 0
     tied = {e.name: e.alias_of for e in plan.entries if e.source == "alias"}  # (one tensor, its first name's layout)
     for world in worlds:
-        parts = [evaluate(plan, (r, world), placements) for r in range(world)]
+        parts = [O.evaluate_plan(plan, SEED, OFFSET, shard=(r, world), placements=placements) for r in range(world)]
         for r, (got, e_end, windows) in enumerate(parts):
             assert e_end == end  # every rank advances its generator identically
             n_windows += windows
@@ -142,7 +84,7 @@ def test_tp_blocks_are_chunks_of_the_eager_model(case, dtype, tmp_path):
     plan = plan_of(case, dtype, tmp_path)  # (through the JSON file)
     placements = tp_placements(deferred_init(lambda: cases.build(case, dtype)), MODELS[case]())
     assert {d for d in placements.values()} == {0, 1, None} if case == "family_opt" else {0, 1}
-    whole, end, _ = evaluate(plan)
+    whole, end, _ = O.evaluate_plan(plan, SEED, OFFSET)
     own, wide = eager(case, dtype)
     compare_with_eager(plan, whole, own, wide)  # the unsharded restatement is the eager model
     assert check_blocks(plan, placements, whole, end) > 0  # (Rowwise weights: windowed descriptors)
@@ -171,7 +113,7 @@ def test_three_dims_unaligned_ragged_and_empty_ranks(dtype, placements, tmp_path
     plan = InitPlan.from_module(deferred_init(lambda: Geometry().to(dtype)))
     plan.save(str(tmp_path / "p.json"))
     plan = InitPlan.load(str(tmp_path / "p.json"))
-    whole, end, _ = evaluate(plan)
+    whole, end, _ = O.evaluate_plan(plan, SEED, OFFSET)
     check_blocks(plan, placements, whole, end, worlds=(2, 3, 4, 8))
 
 
@@ -203,7 +145,7 @@ def test_copy_programs_under_shard_1_are_built_whole_and_narrowed(dtype):
     assert placements == {"pos.weight": 1, "lin.weight": 1, "lin.bias": None}
     entries = {e.name: e for e in plan.entries}
     assert all(narrowed(entries[k], (0, 3), 1) for k in ("pos.weight", "lin.weight"))
-    whole, end, _ = evaluate(plan)
+    whole, end, _ = O.evaluate_plan(plan, SEED, OFFSET)
     torch.manual_seed(0)
     eager_model = build()
     for k in ("pos.weight", "lin.weight"):  # (copies: bit for bit)
@@ -211,7 +153,7 @@ def test_copy_programs_under_shard_1_are_built_whole_and_narrowed(dtype):
     check_blocks(plan, placements, whole, end, worlds=(2, 3, 8))
     # one rank, or no shard at all: the layout changes nothing (and nothing is narrowed)
     for shard in (None, (0, 1)):
-        got, e_end, _ = evaluate(plan, shard, placements)
+        got, e_end, _ = O.evaluate_plan(plan, SEED, OFFSET, shard=shard, placements=placements)
         assert e_end == end and all(torch.equal(got[k], whole[k]) for k in whole), shard
 
 

@@ -1,7 +1,6 @@
 """Tensor-parallel blocks on the H100: the window kernels against the CPU restatement
-(tests/window_oracle.c) and against the plain kernels' unsharded tensor, and the engine's Shard(d) blocks
+(oracle/tdx_oracle.c) and against the plain kernels' unsharded tensor, and the engine's Shard(d) blocks
 (ranks emulated in one process) against the unsharded materialize_module of the same recording."""
-import ctypes
 import math
 
 import numpy as np
@@ -10,6 +9,7 @@ import torch
 from torch.distributed.tensor.parallel import ColwiseParallel, RowwiseParallel
 
 from oracle import cases
+from oracle import tdx_oracle as O
 from torchdistx_b200 import _C
 from torchdistx_b200 import _cabi as C
 from torchdistx_b200.deferred_init import _tp_slots, deferred_init, last_descriptors, last_materialize_stats, \
@@ -17,7 +17,7 @@ from torchdistx_b200.deferred_init import _tp_slots, deferred_init, last_descrip
 from torchdistx_b200.parallel import tp_placements
 from torchdistx_b200.plan import InitPlan
 
-from test_tp_shard_cpu import COPIES_ARGS, COPIES_PLAN, MODELS, Copies, block, oracle
+from test_tp_shard_cpu import COPIES_ARGS, COPIES_PLAN, MODELS, Copies, block
 
 pytestmark = pytest.mark.gpu
 TORCH = {C.TDX_F32: torch.float32, C.TDX_BF16: torch.bfloat16, C.TDX_F16: torch.float16}
@@ -72,10 +72,7 @@ def test_window_kernel_against_the_restatement_and_the_plain_kernel(dt, src, alg
         want = whole.view(rows, cols)[:, c0:c0 + ncol].reshape(-1)[:n]
         assert torch.equal(got.view(torch.uint8), want.contiguous().view(torch.uint8))
     d = window(out, dt, src, c0, n, ncol, cols, **kw)
-    isz = out.element_size()
-    exp = np.empty(n * isz, dtype=np.uint8)
-    assert oracle().tdx_oracle_window_generate(ctypes.byref(d), exp.ctypes.data_as(ctypes.c_void_p)) == 0
-    e = torch.from_numpy(exp).view(TORCH[dt]).double()
+    e = torch.from_numpy(O.generate(d).view(np.uint8)).view(TORCH[dt]).double()
     g = got.cpu().double()
     if src == C.TDX_SRC_UNIFORM and not EPIS[epi]:
         assert torch.equal(g, e)

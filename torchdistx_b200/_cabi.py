@@ -22,6 +22,8 @@ LIB_PATH = os.environ.get("TDX_INIT_LIB") or os.path.join(_HERE, "libtdx_init.so
 # enums of tdx_init.h
 TDX_F32, TDX_BF16, TDX_F16, TDX_I64 = 0, 1, 2, 3
 TDX_RAW8, TDX_RAW16, TDX_RAW32, TDX_RAW64 = 8, 9, 10, 11
+# bytes per element of each dtype
+ITEMSIZE = {TDX_F32: 4, TDX_BF16: 2, TDX_F16: 2, TDX_I64: 8, TDX_RAW8: 1, TDX_RAW16: 2, TDX_RAW32: 4, TDX_RAW64: 8}
 TDX_SRC_CONST, TDX_SRC_UNIFORM, TDX_SRC_NORMAL, TDX_SRC_IOTA = 0, 1, 2, 3
 TDX_SRC_SINCOS = 4
 TDX_SRC_GATHER = 5

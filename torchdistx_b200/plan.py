@@ -713,9 +713,7 @@ class InitPlan:
 def host_staging_bytes(descs, staging_bytes: int = HOST_STAGING_BYTES) -> int:
     """The staging buffer :func:`submit_host` allocates for `descs`: `staging_bytes`, or less when the
     whole table (its bytes, each piece's alignment and the workspace of one pass) fits in less."""
-    item = {_cabi.TDX_F32: 4, _cabi.TDX_BF16: 2, _cabi.TDX_F16: 2, _cabi.TDX_I64: 8, _cabi.TDX_RAW8: 1,
-            _cabi.TDX_RAW16: 2, _cabi.TDX_RAW32: 4, _cabi.TDX_RAW64: 8}
-    data = sum(int(d.elem_count) * item[int(d.dtype)] + 16 for d in descs)
+    data = sum(int(d.elem_count) * _cabi.ITEMSIZE[int(d.dtype)] + 16 for d in descs)
     return min(int(staging_bytes), data + _cabi.load().tdx_init_workspace_bytes(3 * len(descs)))
 
 
